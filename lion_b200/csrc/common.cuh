@@ -69,7 +69,6 @@ struct Ctx {
   unsigned generation = 0;   // bumped whenever the arena / zero grid moves: graphs captured before are stale
   std::mutex* mu = nullptr;  // one forward at a time per context (ctypes releases the GIL); owned by LionCtx
   bool dry = false;
-  bool pdl = false;          // programmatic dependent launch (LION_PDL=1 enables; measured: no gain in graphs)
   int launches = 0;          // kernels launched by the last real pass (gpu_launches evidence)
   // > 0 while side-stream kernels (FPS, neighbour searches) are expected in flight: persistent convolution CTAs then
   // leave this much shared memory unclaimed so that both can be resident on one SM (see conv_tc_run)
@@ -96,28 +95,16 @@ struct Ctx {
 
 int ctx_reserve(Ctx* c, size_t bytes);   // grow arena (sync; not capturable)
 
-// launch helper: skipped in dry mode; counts launches.  With Ctx::pdl (LION_PDL=1) kernels are
-// launched with programmatic stream serialization: every kernel starts with pdl_prologue()
-// (launch_dependents, then wait for the previous kernel to complete and flush).  Off by default:
-// inside the CUDA-graph-captured step the time is the sum of kernel times, not of launch gaps.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(cudaStream_t stream, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-#define LION_LAUNCH(ctx, kernel, grid, block, smem, ...)                               \
+// launch helpers of a forward: skipped in dry mode, counted in Ctx::launches.  LION_LAUNCH uses the context's stream,
+// LION_LAUNCH_ON the given one (the side stream).
+#define LION_LAUNCH_ON(ctx, stream, kernel, grid, block, smem, ...)                    \
   do {                                                                                 \
     if (!(ctx)->dry) {                                                                 \
-      if ((ctx)->pdl) lion::launch_pdl((ctx)->stream, kernel, dim3(grid), dim3(block), (size_t)(smem), __VA_ARGS__); \
-      else kernel<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);            \
+      kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__);                      \
       (ctx)->launches++;                                                               \
     }                                                                                  \
   } while (0)
+#define LION_LAUNCH(ctx, kernel, grid, block, smem, ...) LION_LAUNCH_ON(ctx, (ctx)->stream, kernel, grid, block, smem, __VA_ARGS__)
 
 static __global__ void k_stamp(unsigned long long* p) {
   unsigned long long t;
@@ -132,11 +119,12 @@ inline void stamp(Ctx* c, cudaStream_t s, const char* name, int idx = -1) {
   c->n_stamps++;
 }
 
-inline int memset_async(Ctx* c, void* p, int v, size_t bytes) {
+inline int memset_async(Ctx* c, void* p, int v, size_t bytes, cudaStream_t s) {
   if (c->dry || bytes == 0) return 0;
-  LION_CHECK_CUDA(cudaMemsetAsync(p, v, bytes, c->stream));
+  LION_CHECK_CUDA(cudaMemsetAsync(p, v, bytes, s));
   return 0;
 }
+inline int memset_async(Ctx* c, void* p, int v, size_t bytes) { return memset_async(c, p, v, bytes, c->stream); }
 inline int memcpy_d2d(Ctx* c, void* d, const void* s, size_t bytes) {
   if (c->dry || bytes == 0) return 0;
   LION_CHECK_CUDA(cudaMemcpyAsync(d, s, bytes, cudaMemcpyDeviceToDevice, c->stream));
@@ -173,11 +161,6 @@ static inline size_t cdivz(size_t a, size_t b) { return (a + b - 1) / b; }
 // device utilities
 // ---------------------------------------------------------------------------------------
 #ifdef __CUDACC__
-// PDL prologue of every kernel (see LION_LAUNCH): no global memory access may precede it.
-__device__ __forceinline__ void pdl_prologue() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -27,7 +27,6 @@
 #include "common.cuh"
 #include "model.cuh"
 #include "wgmma.cuh"
-#include <cstdlib>
 
 namespace lion {
 namespace tc {
@@ -97,7 +96,6 @@ template <int KG, int TPG, int NT>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   constexpr int GT = tiles_per_item(NT);
   constexpr int NACC = NT / 2;                  // accumulator registers per thread and tile
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // PDL: see LION_LAUNCH
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* sA = smem;
   const int A_STAGES = P.a_stages;
@@ -126,9 +124,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy zero fill -> async proxy readers
   __syncthreads();
-  // everything above touched only shared memory and overlapped the previous kernel's
-  // tail; from here on global memory written by that kernel is consumed
-  asm volatile("griddepcontrol.wait;" ::: "memory");
 
   // Work distribution.  The (n-tile, shape, row-tile) space is flattened (row tile fastest) and cut into work items = up to G
   // consecutive row tiles sharing the weight slabs (they may belong to two shapes, never to two n-tiles).  Every CTA gets
@@ -425,7 +420,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
 //   w[nt][chunk][tg][t][kg][n][4]  (tf32-rounded, round-to-nearest-away like cuDNN's conversion)
 __global__ void k_pack_tc(const float* __restrict__ wt, float* __restrict__ w, int ntaps, int cin_pad, int cout_pad,
                           int NT, int nchunk, int ntg, int tpg, int KG) {
-  pdl_prologue();
   size_t total = (size_t)(cout_pad / NT) * nchunk * ntg * tpg * KG * NT * 4;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -448,15 +442,6 @@ __global__ void k_pack_tc(const float* __restrict__ wt, float* __restrict__ w, i
 
 }  // namespace tc
 
-static int tc_mode() {      // 1 = tensor cores (default), 0 = SIMT only (LION_CONV_IMPL=simt; bring-up/debug)
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("LION_CONV_IMPL");
-    mode = (e && strcmp(e, "simt") == 0) ? 0 : 1;
-  }
-  return mode;
-}
-
 static void tc_shape(const ConvW& w, int& NT, int& KG, int& nchunk, int& ntg, int& tpg) {
   NT = w.cout_pad < 128 ? w.cout_pad : 128;
   ntg = w.ntaps == 27 ? 3 : 1;
@@ -468,8 +453,6 @@ static void tc_shape(const ConvW& w, int& NT, int& KG, int& nchunk, int& ntg, in
   // 1x1: 32-channel chunks.
   if (w.ntaps == 27) KG = (NT > 64) ? 4 : 8;
   else KG = 8;
-  { static int kg64 = -1; if (kg64 < 0) { const char* e = getenv("LION_TC_KG64"); kg64 = e ? atoi(e) : 0; }
-    if (kg64 && w.ntaps == 27 && NT == 64) KG = kg64; }
   if (G < KG) KG = (G <= 2) ? 2 : ((G <= 4) ? 4 : 8);
   nchunk = (G + KG - 1) / KG;
 }
@@ -501,7 +484,7 @@ int conv_tc_pack_job(const PackJob& j) {
 }
 
 bool conv_tc_usable(const ConvW& w, const ConvGeom& geo) {
-  if (!tc_mode() || !w.tc.w) return false;
+  if (!w.tc.w) return false;
   if (geo.ntaps != w.ntaps) return false;
   return true;
 }
@@ -538,20 +521,16 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   int n_tiles_n = w.cout_pad / NT;
   // row tiles per work item: as many as the accumulator registers hold (the weight slab of a stage is then shared by
   // that many MMA groups); parallelism does not depend on G -- the kernel cuts the flat tile space into equal ranges per CTA
-  int G = tc::tiles_per_item(NT);
-  { static int ge = -1; if (ge < 0) { const char* e = getenv("LION_TC_G"); ge = e ? atoi(e) : 0; } if (ge > 0 && ge < G) G = ge; }
-  P.G = G;
+  P.G = tc::tiles_per_item(NT);
   P.B = B;
   // Round-based items (sched 1) for 3x3x3 grids whose input is well beyond the L2: the three x-plane sweeps of a tile then
   // hit the L2 instead of re-reading DRAM.  Measured on an H100 SXM (400 W, B = 32, kernel alone, sched 0 / 1 alternated
   // twice): every grid above 1.6x the 50 MB L2 runs faster with rounds (64 ch @ 32^3, 322 MB: 7-9 %; 32 ch @ 32^3,
   // 161 MB: 3-4 %; the two 128-channel grids @ 16^3, 95 MB: 5-8 %); below it the two are within about 2 % either way
-  // (one pair of runs of one 25 MB grid excepted), and one contiguous range per CTA is kept.  LION_CONV_SCHED=0|1 forces.
-  { static int sc = -2; if (sc == -2) { const char* e = getenv("LION_CONV_SCHED"); sc = e ? atoi(e) : -1; }
-    const double in_bytes = (double)B * Gin * geo.rows * 16.0;
-    P.sched = sc >= 0 ? sc : (w.ntaps == 27 && in_bytes > 1.6 * c->l2_bytes ? 1 : 0); }
+  // (one pair of runs of one 25 MB grid excepted), and one contiguous range per CTA is kept.
+  const double in_bytes = (double)B * Gin * geo.rows * 16.0;
+  P.sched = w.ntaps == 27 && in_bytes > 1.6 * c->l2_bytes ? 1 : 0;
   P.occ = geo.occ; P.occ_stride = geo.occ_stride;
-  { static int ns = -1; if (ns < 0) { const char* e = getenv("LION_TC_NOSKIP"); ns = e ? atoi(e) : 0; } if (ns) P.occ = nullptr; }
   const size_t fixed = tc::smem_fixed(NT, tpg);
   long long room = 227LL * 1024 - (long long)fixed - (long long)tc::B_STAGES * P.b_stage_bytes;
   int a_stages = (int)(room / P.a_stage_bytes);
@@ -566,7 +545,6 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
     if (capped >= 4 && capped < a_stages) a_stages = capped;
   }
   if (a_stages > tc::MAX_A_STAGES) a_stages = tc::MAX_A_STAGES;
-  { static int as = -1; if (as < 0) { const char* e = getenv("LION_TC_ASTAGES"); as = e ? atoi(e) : 0; } if (as > 0 && as < a_stages) a_stages = as; }
   if (a_stages < 2) { set_error("conv_tc: shared memory cannot hold the operand pipeline (N=%d, KG=%d)", NT, KG); return LION_ERR_ARG; }
   P.a_stages = a_stages;
   size_t smem = (size_t)a_stages * P.a_stage_bytes + (size_t)tc::B_STAGES * P.b_stage_bytes + fixed;
@@ -577,7 +555,7 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   long long n_units = (long long)ntile * n_tiles_n * B;
   long long per_cta = (n_units + c->num_sms - 1) / c->num_sms;
   int grid = (int)((n_units + per_cta - 1) / per_cta);
-#define LION_TC_CASE(kg, tpg_, nt_)                                                                       \
+#define CONV_TC_CASE(kg, tpg_, nt_)                                                                       \
   if (KG == kg && tpg == tpg_ && NT == nt_) {                                                             \
     static DevOnce attr_once;                                                                             \
     if (attr_once.need()) {                                                                               \
@@ -586,10 +564,10 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
     LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_>), grid, tc::THREADS, smem, P);                           \
     return check_launch(c, "conv_tc");                                                                    \
   }
-#define LION_TC_NT(kg, tpg_) LION_TC_CASE(kg, tpg_, 32) LION_TC_CASE(kg, tpg_, 64) LION_TC_CASE(kg, tpg_, 96) LION_TC_CASE(kg, tpg_, 128)
-  LION_TC_NT(2, 1) LION_TC_NT(4, 1) LION_TC_NT(8, 1) LION_TC_NT(2, 9) LION_TC_NT(4, 9) LION_TC_NT(8, 9)
-#undef LION_TC_NT
-#undef LION_TC_CASE
+#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32) CONV_TC_CASE(kg, tpg_, 64) CONV_TC_CASE(kg, tpg_, 96) CONV_TC_CASE(kg, tpg_, 128)
+  CONV_TC_NT(2, 1) CONV_TC_NT(4, 1) CONV_TC_NT(8, 1) CONV_TC_NT(2, 9) CONV_TC_NT(4, 9) CONV_TC_NT(8, 9)
+#undef CONV_TC_NT
+#undef CONV_TC_CASE
   set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps", NT, KG, tpg);
   return LION_ERR_ARG;
 }

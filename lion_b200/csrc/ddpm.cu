@@ -20,7 +20,6 @@ namespace lion {
 __global__ void k_ddpm_update(const float* x /* may alias xo (in-place update) */, const float* __restrict__ eps, const float* __restrict__ noise,
                               float* xo, const float4* __restrict__ tables, const int* __restrict__ step,
                               float temp, size_t n, float* __restrict__ hist, int T) {
-  pdl_prologue();
   int t = *step;
   float4 c = tables[t];
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -41,14 +40,12 @@ __global__ void k_ddpm_update(const float* x /* may alias xo (in-place update) *
 // (given_noise: host noise uploaded ahead of the loop) keep the copy INSIDE the captured step graph, selected by the same
 // device-side step counter as the update's table row: no per-step host work besides the graph replay.
 __global__ void k_ddpm_fetch_noise(float4* __restrict__ dst, const float4* __restrict__ block, const int* __restrict__ step, size_t n4) {
-  pdl_prologue();
   const int t = *step;
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n4) dst[i] = block[(size_t)t * n4 + i];
 }
 
 __global__ void k_ddpm_set_step(int* step, float* t_out, int B, int t_index, int advance) {
-  pdl_prologue();
   int t = advance ? (*step - 1) : t_index;
   __syncthreads();
   if (threadIdx.x == 0) *step = t;
@@ -62,7 +59,6 @@ __global__ void k_ddpm_set_step(int* step, float* t_out, int B, int t_index, int
 __global__ void k_ddim_update(const float* x /* may alias xo (in-place update) */, const float* __restrict__ eps, const float* __restrict__ noise,
                               float* xo, const float4* __restrict__ tables, const int* __restrict__ step,
                               size_t n, float* __restrict__ hist) {
-  pdl_prologue();
   int s = *step;
   float4 c = tables[s];
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -75,7 +71,6 @@ __global__ void k_ddim_update(const float* x /* may alias xo (in-place update) *
 
 // step index i -> i+1 (or set), and the model's timestep vector t_out[b] = tables[i].w
 __global__ void k_ddim_set_step(int* step, float* t_out, const float4* __restrict__ tables, int B, int S, int index, int advance) {
-  pdl_prologue();
   int s = advance ? (*step + 1) : index;
   __syncthreads();
   if (threadIdx.x == 0) *step = s;
@@ -91,7 +86,6 @@ __global__ void k_ddim_set_step(int* step, float* t_out, const float4* __restric
 // table row t (8 floats): { sqrt(1-abar_t), sqrt(abar_t), c0, c1, sqrt(var_t), 0, 0, 0 }.
 __global__ void k_sched_step(const float* x /* may alias xo (in-place update) */, const float* __restrict__ eps, const float* __restrict__ noise,
                              float* xo, const float4* __restrict__ tables, const int* __restrict__ step, size_t n) {
-  pdl_prologue();
   int t = *step;
   float4 c = tables[2 * t];
   float sigma = tables[2 * t + 1].x;

@@ -60,7 +60,6 @@ struct GpEpi {
 __global__ void __launch_bounds__(GP_WARPS * 32, 1)
 k_gp_partial(const float* __restrict__ W, const float* __restrict__ x, int x_stride, const float* __restrict__ add,
              int add_stride, float* __restrict__ part, int B, int K, int O, GpEpi epi) {
-  pdl_prologue();
   extern __shared__ __align__(16) float s_mem[];
   float* s_w = s_mem;                          // [GP_OB][GP_PITCH]
   float* s_x = s_mem + GP_OB * GP_PITCH;       // [GP_BT][GP_PITCH]
@@ -158,7 +157,6 @@ k_gp_partial(const float* __restrict__ W, const float* __restrict__ x, int x_str
 __global__ void k_gp_reduce(const float* __restrict__ part, int nsplit, const float* __restrict__ bias, float* __restrict__ out,
                             int out_stride, const float* __restrict__ mul, int mul_stride, const float* __restrict__ res,
                             int res_stride, int B, int O, int act) {
-  pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * O) return;
   int b = i / O, o = i % O;
@@ -179,7 +177,6 @@ __global__ void k_gp_reduce(const float* __restrict__ part, int nsplit, const fl
 // PositionalEmbedding (models/utils.py:16-31): fp32 frequencies exp(i * -log(1e4)/(half-1))
 __global__ void k_gp_posemb(const float* __restrict__ t, const float* __restrict__ freqs, float* __restrict__ out,
                             int half, float scale) {
-  pdl_prologue();
   int b = blockIdx.x, i = threadIdx.x;
   if (i >= half) return;
   float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);

@@ -30,7 +30,6 @@ constexpr int CD_CHUNK = 2048;     // candidates staged per pass (24 KB)
 __global__ void __launch_bounds__(CD_THREADS)
 k_chamfer_nn(const float* __restrict__ q, const float* __restrict__ c, float* __restrict__ dist, int* __restrict__ idx,
              int n, int m) {
-  pdl_prologue();
   __shared__ float sx[CD_CHUNK], sy[CD_CHUNK], sz[CD_CHUNK];
   const int b = blockIdx.y;
   const float* qb = q + (size_t)b * n * 3;
@@ -109,7 +108,6 @@ __device__ __forceinline__ float cd_direction_sum(const float* qx, const float* 
 __global__ void __launch_bounds__(CD_PW_THREADS)
 k_chamfer_pairwise(const float* __restrict__ samples, const float* __restrict__ refs, float* __restrict__ out,
                    int n, int m, int n_ref) {
-  pdl_prologue();
   extern __shared__ float sm[];     // s: x,y,z [n] ; r: x,y,z [m] ; reduction scratch
   float* sxp = sm; float* syp = sxp + CD_PW_MAX; float* szp = syp + CD_PW_MAX;
   float* rxp = szp + CD_PW_MAX; float* ryp = rxp + CD_PW_MAX; float* rzp = ryp + CD_PW_MAX;
@@ -193,7 +191,6 @@ __device__ __forceinline__ float emd_d2(float x1, float y1, float z1, float x2, 
 // pair p: xyz1 = a[(p / nb) or p], xyz2 = b[(p % nb) or p]
 __global__ void __launch_bounds__(EMD_THREADS)
 k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* __restrict__ out, int n, int m, int nb, int pairwise) {
-  pdl_prologue();
   extern __shared__ float sm[];
   float4* p1 = reinterpret_cast<float4*>(sm);            // [n] x,y,z of xyz1 + ratioL
   float4* p2 = p1 + EMD_MAX;                             // [m] x,y,z of xyz2 + (remainR | ratioR)

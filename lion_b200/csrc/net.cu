@@ -85,7 +85,6 @@ int ctx_reserve_zgrid(Ctx* c, size_t bytes) {
 // weight packing kernels
 __global__ void k_pack_conv_w(const float* __restrict__ w_ref, const int* __restrict__ kmap, float* __restrict__ wt,
                               int ntaps, int cin_ref, int cin_pad, int cout, int cout_pad) {
-  pdl_prologue();
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)ntaps * cin_pad * cout_pad;
   if (i >= total) return;
@@ -99,7 +98,6 @@ __global__ void k_pack_conv_w(const float* __restrict__ w_ref, const int* __rest
 }
 // sparse first convolution: the 27 taps side by side, wy[ci][t * cout_pad + co] = wt[t][ci][co] (zero beyond 27 * cout_pad)
 __global__ void k_pack_taps_wide(const float* __restrict__ wt, float* __restrict__ wy, int cin_pad, int cout_pad, int ny_pad) {
-  pdl_prologue();
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)cin_pad * ny_pad) return;
   int n = i % ny_pad, ci = i / ny_pad;
@@ -107,7 +105,6 @@ __global__ void k_pack_taps_wide(const float* __restrict__ wt, float* __restrict
   wy[i] = t < 27 ? wt[((size_t)t * cin_pad + ci) * cout_pad + co] : 0.0f;
 }
 __global__ void k_pad_vec(const float* __restrict__ src, float* __restrict__ dst, int n, int n_pad) {
-  pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_pad) dst[i] = i < n ? src[i] : 0.0f;
 }
@@ -441,13 +438,12 @@ static int attn_fwd(Fwd& f, const AttnBlk& a, PF x, float4* dst, int Gd, int g_o
 // The first convolution of a PVConv reads a grid with at most N occupied voxels.  When that is a small fraction of r^3
 // (<= 25 %) it is cheaper to multiply only the occupied voxels by all 27 taps (one GEMM, 27 * N rows of output instead of r^3 * 27
 // taps of dense work) and let every output voxel gather its neighbours' rows (k_sparse_conv_gather): at r = 32, N = 2048
-// that is 16x fewer FLOPs and the convolution becomes a ~0.7 GB streaming problem.  LION_SPARSE_CONV1=0 disables it.
+// that is 16x fewer FLOPs and the convolution becomes a ~0.7 GB streaming problem.
 static bool sparse_conv1_wanted(int N, int r) {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("LION_SPARSE_CONV1"); on = e ? atoi(e) : 1; }
-  return on && (long long)N * 4 <= (long long)r * r * r;
+  return (long long)N * 4 <= (long long)r * r * r;
 }
-static int get_vox(Fwd& f, const float4* c4, int N, int r, VoxPrep** out) {
+// voxelisation prep of the points c4 at resolution r, launched on stream s (once per forward: later calls find it)
+static int get_vox(Fwd& f, cudaStream_t s, const float4* c4, int N, int r, VoxPrep** out) {
   for (auto& v : f.vox) if (v.c4 == c4 && v.N == N && v.r == r) { *out = &v; return 0; }
   VoxPrep v{c4, N, r, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr};
   if (N > VOXP_MAXN || r > 32) { set_error("voxelisation: N=%d (max %d) or r=%d (max 32) unsupported", N, VOXP_MAXN, r); return LION_ERR_ARG; }
@@ -458,14 +454,15 @@ static int get_vox(Fwd& f, const float4* c4, int N, int r, VoxPrep** out) {
   int P = (r + 2) * (r + 2) * (r + 2);
   v.occ_stride = (P + 63) / 64 + 4;
   v.occ = f.c->alloc_n<unsigned char>((size_t)f.B * v.occ_stride);
-  LION_TRY(memset_async(f.c, v.occ, 0, (size_t)f.B * v.occ_stride));
+  LION_TRY(memset_async(f.c, v.occ, 0, (size_t)f.B * v.occ_stride, s));
   if (sparse_conv1_wanted(N, r)) {
     v.cidx = f.c->alloc_n<int>((size_t)f.B * N);
     v.nocc = f.c->alloc_n<int>((size_t)f.B);
     v.vgrid = f.c->alloc_n<int>((size_t)f.B * P);
-    LION_TRY(memset_async(f.c, v.vgrid, 0xff, (size_t)f.B * P * sizeof(int)));     // -1 = empty voxel
+    LION_TRY(memset_async(f.c, v.vgrid, 0xff, (size_t)f.B * P * sizeof(int), s));     // -1 = empty voxel
   }
-  LION_LAUNCH(f.c, k_vox_prep, f.B, VOXP_THREADS, 0, c4, v.nc, v.order, v.ppos, v.len, v.occ, v.occ_stride, N, r, v.cidx, v.nocc, v.vgrid);
+  LION_LAUNCH_ON(f.c, s, k_vox_prep, f.B, VOXP_THREADS, 0, c4, v.nc, v.order, v.ppos, v.len, v.occ, v.occ_stride, N, r, v.cidx, v.nocc,
+                 v.vgrid);
   LION_TRY(check_launch(f.c, "vox_prep"));
   f.vox.push_back(v);
   *out = &f.vox.back();
@@ -477,12 +474,10 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
   if (feat.G != Gin) { set_error("PVConv: got %d input channels, expected %d", feat.G * 4, p.cin); return LION_ERR_ARG; }
   VoxPrep* vp;
-  LION_TRY(get_vox(f, c4, N, r, &vp));
+  LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
   size_t mk = f.c->mark();
   ConvGeom geo = geom_grid(r);
-  static int sparse_minc = -1;
-  if (sparse_minc < 0) { const char* e = getenv("LION_SPARSE_MINC"); sparse_minc = e ? atoi(e) : 32; }
-  const bool sparse1 = vp->cidx && ygemm_usable(p.c1y) && feat.G == p.c1y.cin_pad / 4 && p.c1.cout_pad >= sparse_minc;
+  const bool sparse1 = vp->cidx && ygemm_usable(p.c1y) && feat.G == p.c1y.cin_pad / 4;
   float4* g_in = nullptr;
   PF xc;
   if (sparse1) {
@@ -579,6 +574,27 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   return 0;
 }
 
+// furthest-point sampling of M centres (and their indices) out of N packed points per shape, on stream s
+template <int A, int C, bool FULL>
+static int fps_c4_on(Ctx* c, cudaStream_t s, int B, const float4* c4, int* fidx, float4* centers, int N, int M, int VT) {
+  static DevOnce attr_once;
+  if (attr_once.need()) {
+    LION_CHECK_CUDA(cudaFuncSetAttribute(k_fps_c4<A, C, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fps_smem_bytes(FPS_MAX_N)));
+    // FPS runs on the side stream next to the convolutions: same (maximum) carve-out as theirs (see unet_forward)
+    LION_CHECK_CUDA(cudaFuncSetAttribute(k_fps_c4<A, C, FULL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  }
+  LION_LAUNCH_ON(c, s, (k_fps_c4<A, C, FULL>), B, FPS_THREADS, fps_smem_bytes(N), c4, fidx, centers, N, M, VT);
+  return 0;
+}
+static int fps_c4(Ctx* c, cudaStream_t s, int B, const float4* c4, int* fidx, float4* centers, int N, int M) {
+  const int VT = fps_virtual_threads(N);
+  int rc = 0;
+#define LION_FPS_CALL(A_, C_, F_) rc = fps_c4_on<A_, C_, F_>(c, s, B, c4, fidx, centers, N, M, VT)
+  LION_FPS_DISPATCH(N, VT, LION_FPS_CALL);
+#undef LION_FPS_CALL
+  return rc;
+}
+
 // SA module: (features PF, coords) -> (dst PF with Gd groups at g_off, centres C4)
 // pre_fps >= 0: the centres were already sampled on the side stream (event ev[pre_fps])
 static int sa_fwd(Fwd& f, const SABlk& s, PF feat, const float4* c4, float4* centers, float4* dst, int Gd, int g_off,
@@ -592,15 +608,7 @@ static int sa_fwd(Fwd& f, const SABlk& s, PF feat, const float4* c4, float4* cen
     if (!f.c->dry) LION_CHECK_CUDA(cudaStreamWaitEvent(f.c->stream, f.c->ev[pre_fps], 0));
   } else {
     int* fidx = f.c->alloc_n<int>((size_t)f.B * M);
-    const int VT = fps_virtual_threads(N);
-#define LION_FPS_CALL(A_, C_, F_)                                                                                         \
-  do {                                                                                                                    \
-    if (fps_smem_bytes(N) > 48 * 1024)                                                                                    \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(k_fps_c4<A_, C_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); \
-    LION_LAUNCH(f.c, (k_fps_c4<A_, C_, F_>), f.B, FPS_THREADS, fps_smem_bytes(N), c4, fidx, centers, N, M, VT);           \
-  } while (0)
-    LION_FPS_DISPATCH(N, VT, LION_FPS_CALL);
-#undef LION_FPS_CALL
+    LION_TRY(fps_c4(f.c, f.c->stream, f.B, c4, fidx, centers, N, M));
   }
   const int* nidx = pre_nidx;                     // ball query already ran on the side stream (behind event ev[pre_fps])
   if (!nidx) {
@@ -770,7 +778,6 @@ static int build_unet(Model* m, Cursor& cur) {
 }
 
 __global__ void k_extract_extra(const float4* __restrict__ x, float4* __restrict__ o, int total) {
-  pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < total) o[i] = make_float4(x[i].w, 0.f, 0.f, 0.f);
 }
@@ -890,10 +897,8 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
   // bound rounds on 32 SMs.  Fork it onto the side stream so it hides under the first PVConvs.
   std::vector<float4*> fps_centers(n_sa, nullptr);
   // Neighbour searches depend on coordinates only as well: the ball query of level i follows FPS i on the side stream,
-  // the four 3-NN searches of the FP half follow the last FPS (LION_AUX_NN=0: keep them on the main stream).
-  static int aux_nn = -1;
-  if (aux_nn < 0) { const char* e = getenv("LION_AUX_NN"); aux_nn = e ? atoi(e) : 1; }
-  const bool side_nn = aux_nn != 0 && n_sa <= 4;
+  // the four 3-NN searches of the FP half follow the last FPS.
+  const bool side_nn = n_sa <= 4;
   std::vector<int*> sa_nidx(n_sa, nullptr), fp_idx(n_sa, nullptr);
   std::vector<char> vox_pending(n_sa + 1, 0);
   std::vector<float*> fp_wgt(n_sa, nullptr);
@@ -914,40 +919,25 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
       if (ncur > FPS_MAX_N || sb.m > ncur) { set_error("unet: FPS sizes unsupported"); return LION_ERR_ARG; }
       fps_centers[i] = c->alloc_n<float4>((size_t)B * sb.m);
       int* fidx = c->alloc_n<int>((size_t)B * sb.m);
-      if (!c->dry) {
-        const int VT = fps_virtual_threads(ncur);
-#define LION_FPS_CALL(A_, C_, F_)                                                                                         \
-  do {                                                                                                                    \
-    if (fps_smem_bytes(ncur) > 48 * 1024)                                                                                 \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(k_fps_c4<A_, C_, F_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); \
-    LION_CHECK_CUDA(cudaFuncSetAttribute(k_fps_c4<A_, C_, F_>, cudaFuncAttributePreferredSharedMemoryCarveout,            \
-                                         cudaSharedmemCarveoutMaxShared));                                               \
-    k_fps_c4<A_, C_, F_><<<B, FPS_THREADS, fps_smem_bytes(ncur), c->aux>>>(src, fidx, fps_centers[i], ncur, sb.m, VT);    \
-  } while (0)
-        LION_FPS_DISPATCH(ncur, VT, LION_FPS_CALL);
-#undef LION_FPS_CALL
-        c->launches++;
-        stamp(c, c->aux, "aux:fps", i);
-      }
+      LION_TRY(fps_c4(c, c->aux, B, src, fidx, fps_centers[i], ncur, sb.m));
+      stamp(c, c->aux, "aux:fps", i);
       if (side_nn) {
         sa_nidx[i] = c->alloc_n<int>((size_t)B * sb.m * sb.k);
-        if (!c->dry) {
-          k_ball_query_c4<<<dim3(cdiv(sb.m * 32, 256), B), 256, 0, c->aux>>>(fps_centers[i], src, sa_nidx[i], ncur, sb.m,
-                                                                             sb.radius * sb.radius, sb.k);
-          c->launches++;
-          stamp(c, c->aux, "aux:ballq", i);
-        }
+        LION_LAUNCH_ON(c, c->aux, k_ball_query_c4, dim3(cdiv(sb.m * 32, 256), B), 256, 0, fps_centers[i], src, sa_nidx[i], ncur, sb.m,
+                       sb.radius * sb.radius, sb.k);
+        stamp(c, c->aux, "aux:ballq", i);
       }
       if (!c->dry) LION_CHECK_CUDA(cudaEventRecord(c->ev[i], c->aux));
-      if (i == 0 && temb && !c->dry) {
+      if (i == 0 && temb) {
         // three tiny dependent launches (~45 us of latency) that nothing needs before level 1
-        k_time_sinusoid<<<B, 64, 0, c->aux>>>(t, u.d_freqs, temb_sinu, E / 2, 1.0f);
-        k_small_linear<<<B, 128, E * sizeof(float), c->aux>>>(u.e0w, u.e0b, temb_sinu, E, temb_h, E, E, E, 1);
-        k_small_linear<<<B, 128, E * sizeof(float), c->aux>>>(u.e2w, u.e2b, temb_h, E, temb, E, E, E, 0);
-        c->launches += 3;
+        LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, temb_sinu, E / 2, 1.0f);
+        LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e0w, u.e0b, temb_sinu, E, temb_h, E, E, E, 1);
+        LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e2w, u.e2b, temb_h, E, temb, E, E, E, 0);
         stamp(c, c->aux, "aux:temb");
-        LION_CHECK_CUDA(cudaEventRecord(c->ev_temb, c->aux));
-        temb_pending = true;
+        if (!c->dry) {
+          LION_CHECK_CUDA(cudaEventRecord(c->ev_temb, c->aux));
+          temb_pending = true;
+        }
       }
       // voxelisation prep of the PVConvs that work on these centres (the next SA level and, mirrored, an FP level):
       // it depends on coordinates only -- one CTA per shape, 13-25 us each on the critical path otherwise
@@ -959,12 +949,8 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
         bool any = false;
         for (int k = 0; k < 2; ++k) {
           if (rs[k] <= 0 || (k == 1 && rs[1] == rs[0])) continue;
-          cudaStream_t main_stream = c->stream;
-          c->stream = c->aux;
           VoxPrep* vp = nullptr;
-          int rc = get_vox(f, fps_centers[i], sb.m, rs[k], &vp);
-          c->stream = main_stream;
-          if (rc) return rc;
+          LION_TRY(get_vox(f, c->aux, fps_centers[i], sb.m, rs[k], &vp));
           any = true;
         }
         if (any && !c->dry) {
@@ -982,13 +968,10 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
         const int npts = lvl == 0 ? N : u.sa[lvl - 1].back().sa.m, nctr = u.sa[lvl].back().sa.m;
         fp_idx[lvl] = c->alloc_n<int>((size_t)B * npts * 3);
         fp_wgt[lvl] = c->alloc_n<float>((size_t)B * npts * 3);
-        if (!c->dry) {
-          k_three_nn_c4<<<dim3(cdiv(npts, 128), B), 128, 1024 * sizeof(float4), c->aux>>>(pts, fps_centers[lvl], fp_idx[lvl],
-                                                                                        fp_wgt[lvl], npts, nctr);
-          c->launches++;
-          stamp(c, c->aux, "aux:3nn", lvl);
-          LION_CHECK_CUDA(cudaEventRecord(c->ev[4 + lvl], c->aux));
-        }
+        LION_LAUNCH_ON(c, c->aux, k_three_nn_c4, dim3(cdiv(npts, 128), B), 128, 1024 * sizeof(float4), pts, fps_centers[lvl], fp_idx[lvl],
+                       fp_wgt[lvl], npts, nctr);
+        stamp(c, c->aux, "aux:3nn", lvl);
+        if (!c->dry) LION_CHECK_CUDA(cudaEventRecord(c->ev[4 + lvl], c->aux));
       }
     }
   }
@@ -1004,10 +987,10 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
     *dstp = d;
     return check_launch(c, "concat temb");
   };
-  static int share_kb = -1;
-  if (share_kb < 0) { const char* e = getenv("LION_TC_SHARE_KB"); share_kb = e ? atoi(e) : 196; }
+  // shared memory a convolution CTA may claim while side-stream kernels are resident on its SM (see conv_tc_run)
+  constexpr int CONV_SMEM_BESIDE_AUX = 196 * 1024;
   for (int i = 0; i < n_sa; ++i) {
-    c->conv_smem_cap = (i == 0 && share_kb > 0) ? share_kb * 1024 : 0;      // the side stream is busy during level 0
+    c->conv_smem_cap = i == 0 ? CONV_SMEM_BESIDE_AUX : 0;      // the side stream is busy during level 0
     feats_list[i] = feat; coords_list[i] = coords; n_list[i] = Ncur;
     if (vox_pending[i]) { LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, c->ev_vox[i - 1], 0)); vox_pending[i] = 0; }
     if (i > 0 && has_t) LION_TRY(with_temb(feat, &feat));
@@ -1121,7 +1104,6 @@ extern "C" int lion_ctx_create(int device, LionCtx** out) {
   LION_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
   h->c.num_sms = prop.multiProcessorCount;
   h->c.l2_bytes = prop.l2CacheSize;
-  { const char* e = getenv("LION_PDL"); h->c.pdl = (e && atoi(e) != 0); }   // measured: no gain inside CUDA graphs; off by default
   LION_CHECK_CUDA(cudaStreamCreateWithFlags(&h->c.aux, cudaStreamNonBlocking));
   { const char* e = getenv("LION_TIMELINE");
     if (e && atoi(e) != 0) LION_CHECK_CUDA(cudaMalloc(&h->c.d_stamps, LION_MAX_STAMPS * sizeof(unsigned long long))); }
@@ -1484,7 +1466,6 @@ extern "C" int lion_global_prior_forward(LionModel* h, const float* x, const flo
 
 // ---- measurement hook: time the convolution kernel alone (bench.py roofline leg) ------------
 __global__ void k_fill_pattern(float* p, size_t n, float scale) {
-  pdl_prologue();
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { unsigned h = (unsigned)(i * 2654435761u) ^ 0x9e3779b9u; h ^= h >> 15; h *= 2246822519u; h ^= h >> 13;
                p[i] = scale * ((float)(h & 0xffff) / 32768.0f - 1.0f); }

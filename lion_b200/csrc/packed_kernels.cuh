@@ -31,7 +31,6 @@ __device__ __forceinline__ float4 f4_fma(float4 a, float s, float4 c) {
 // latent x[B][N][D] (D<=4 floats per point... here D==4) -> C4 coordinates
 // ------------------------------------------------------------------------------------
 __global__ void k_make_coords(const float4* __restrict__ x, float4* __restrict__ c4, int total) {
-  pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   float4 v = x[i];
@@ -54,7 +53,6 @@ __global__ void __launch_bounds__(VOXP_THREADS)
 k_vox_prep(const float4* __restrict__ c4, float4* __restrict__ nc, int* __restrict__ s_order, int* __restrict__ s_ppos,
            int* __restrict__ s_len, unsigned char* __restrict__ occ, int occ_stride, int N, int r,
            int* __restrict__ s_cidx /*[B][N] or null*/, int* __restrict__ nocc /*[B]*/, int* __restrict__ vgrid /*[B][(r+2)^3], pre-set to -1*/) {
-  pdl_prologue();
   int b = blockIdx.x;
   const float4* c = c4 + (size_t)b * N;
   __shared__ float s_stat[4];
@@ -145,7 +143,6 @@ k_vox_prep(const float4* __restrict__ c4, float4* __restrict__ nc, int* __restri
 // summation order as k_scatter); rows n_occ..N-1 are zeroed.
 __global__ void k_scatter_compact(const float4* __restrict__ feat, const int* __restrict__ s_order, const int* __restrict__ s_cidx,
                                   const int* __restrict__ s_len, const int* __restrict__ nocc, float4* __restrict__ xc, int G, int N) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= N) return;
@@ -209,7 +206,6 @@ __global__ void __launch_bounds__(128)
 k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict__ vgrid, const float* __restrict__ bias,
                      float4* __restrict__ out, double* __restrict__ ssum, double* __restrict__ ssq, int stat_stride,
                      int r, int Nrows) {
-  pdl_prologue();
   static_assert(C == 32 || C == 64, "two (or one) channels per lane");
   constexpr int CPL = C / 32;                     // channels per lane
   constexpr int PITCH = C + 2;
@@ -291,7 +287,6 @@ k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict
 // reference does (vox.cu:65-68), and stores once.
 __global__ void k_scatter(const float4* __restrict__ feat, const int* __restrict__ s_order, const int* __restrict__ s_ppos,
                           const int* __restrict__ s_len, float4* __restrict__ grid, int G, int N, int P) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= N) return;
@@ -321,7 +316,6 @@ __global__ void __launch_bounds__(128)
 k_conv_simt(const float4* __restrict__ in, const float* __restrict__ Wt, const float* __restrict__ bias,
             float4* __restrict__ out, double* __restrict__ ssum, double* __restrict__ ssq,
             int Gin, int cin_pad, int cout_pad, int Gout_store, ConvGeom geo) {
-  pdl_prologue();
   extern __shared__ float s_w[];   // [ntaps][4][COT]
   int b = blockIdx.z;
   int co0 = blockIdx.y * COT;
@@ -400,7 +394,6 @@ struct PrepJob {
 // Two layers whose statistics are complete at the same point of the stream (a PVConv's first convolution and its
 // point branch) are folded by ONE launch: each tiny launch costs 4-5 us on the step's critical path.
 __global__ void k_affine_prep(PrepJob j0, PrepJob j1) {
-  pdl_prologue();
   extern __shared__ float s_f[];   // [C] se input, [C/8] hidden
   __shared__ double s_gs[8], s_gq[8];
   const PrepJob& J = blockIdx.y == 0 ? j0 : j1;
@@ -466,7 +459,6 @@ __global__ void k_affine_prep(PrepJob j0, PrepJob j1) {
 // all AdaGN style Linears of a network in one launch: out[b][off_l + o] = W_l[o] . style[b] + bias_l[o]
 __global__ void k_style_linear(const StyleLayer* __restrict__ layers, const float* __restrict__ style, int S,
                                float* __restrict__ out, int out_stride) {
-  pdl_prologue();
   extern __shared__ float s_style[];
   StyleLayer L = layers[blockIdx.x];
   int b = blockIdx.y;
@@ -487,7 +479,6 @@ __global__ void k_style_linear(const StyleLayer* __restrict__ layers, const floa
 
 // max over the rows of a PF: out[b][c] = max_i in[b][c/4][i].c%4   (PointNetPlusEncoder: features.max(-1), shapelatent_modules.py:46)
 __global__ void k_max_rows(const float4* __restrict__ in, float* __restrict__ out, int G, int R) {
-  pdl_prologue();
   int b = blockIdx.y, g = blockIdx.x;
   const float4* src = in + ((size_t)b * G + g) * R;
   float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
@@ -504,13 +495,11 @@ __global__ void k_max_rows(const float4* __restrict__ in, float* __restrict__ ou
 }
 // [B][N][3] -> PF / C4 [B][N] float4 (x, y, z, 0): networks whose points carry no extra feature channel
 __global__ void k_pad3(const float* __restrict__ x, float4* __restrict__ o, int total) {
-  pdl_prologue();
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < total) o[i] = make_float4(x[3 * (size_t)i], x[3 * (size_t)i + 1], x[3 * (size_t)i + 2], 0.0f);
 }
 // PF with G groups -> point-major [B][R][C]
 __global__ void k_pf_to_pm(const float4* __restrict__ src, float* __restrict__ dst, int G, int C, int R) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R) return;
@@ -526,7 +515,6 @@ __global__ void k_pf_to_pm(const float4* __restrict__ src, float* __restrict__ d
 // generic small dense layer on [B][K] rows: out = act(W x + b); act 0 none, 1 leaky(0.1)
 __global__ void k_small_linear(const float* __restrict__ W, const float* __restrict__ bias, const float* __restrict__ x,
                                int x_stride, float* __restrict__ out, int out_stride, int K, int O, int act) {
-  pdl_prologue();
   extern __shared__ float s_x[];
   int b = blockIdx.x;
   for (int i = threadIdx.x; i < K; i += blockDim.x) s_x[i] = x[(size_t)b * x_stride + i];
@@ -548,7 +536,6 @@ __global__ void k_small_linear(const float* __restrict__ W, const float* __restr
 // host in float64 and rounded to fp32 exactly like the reference
 __global__ void k_time_sinusoid(const float* __restrict__ t, const float* __restrict__ freqs, float* __restrict__ out,
                                 int half, float scale) {
-  pdl_prologue();
   int b = blockIdx.x, i = threadIdx.x;
   if (i >= half) return;
   float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);
@@ -607,7 +594,6 @@ constexpr int ACT_U = 4;
 // per PVConv on the critical path); block (x, y, z) zeroes its 256 points in groups y, y + gridDim.y, ... < us_G.
 __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ out, AffSrc aff, int G, int C, int rp, int P,
                            int nb_act, const int* __restrict__ us_ppos, float4* __restrict__ us_grid, int us_G, int us_N) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   if ((int)blockIdx.x >= nb_act) {
     int sidx = ((int)blockIdx.x - nb_act) * blockDim.x + threadIdx.x;
@@ -653,7 +639,6 @@ __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ o
 template <int POOL>
 __global__ void k_act_rows(const float4* __restrict__ in, float4* __restrict__ out, AffSrc aff, int G, int C, int R_out, int Gd,
                            int g_off, int flags) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   float4 s, t;
@@ -674,7 +659,6 @@ __global__ void k_act_rows(const float4* __restrict__ in, float4* __restrict__ o
 // k_act_rows<32>, bit for bit.
 __global__ void k_act_rows_pool32(const float4* __restrict__ in, float4* __restrict__ out, AffSrc aff, int G, int C, int R_out,
                                   int Gd, int g_off) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   float4 s, t;
@@ -709,7 +693,6 @@ __global__ void k_act_rows_pool32(const float4* __restrict__ in, float4* __restr
 // maximum over the neighbours is attained at one of the two extremes: the same set maximum as k_act_rows_pool32.
 __global__ void k_act_pool_minmax(const float4* __restrict__ mm, float4* __restrict__ out, AffSrc aff, int G, int C, int R_out,
                                   int Gd, int g_off) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   float4 s, t;
   aff_block_load(aff, b, g, C, s, t);
@@ -724,7 +707,6 @@ __global__ void k_act_pool_minmax(const float4* __restrict__ mm, float4* __restr
 // on the fused path these statistics come out of the convolution epilogue instead)
 __global__ void k_row_stats(const float4* __restrict__ in, double* __restrict__ ssum, double* __restrict__ ssq, int G, int R,
                             int stat_stride) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R; i += gridDim.x * blockDim.x) {
@@ -745,7 +727,6 @@ __global__ void k_row_stats(const float4* __restrict__ in, double* __restrict__ 
 // SE3d gate from channel means (models/pvcnn2_ada.py:27-41): gate[b][c] = sigmoid(W2 relu(W1 mean)); grid = B, block = C
 __global__ void k_se_gate(const double* __restrict__ ssum, int stat_stride, const float* __restrict__ w1, const float* __restrict__ w2,
                           float* __restrict__ gate, int C, double count) {
-  pdl_prologue();
   extern __shared__ float s_f[];
   int b = blockIdx.x, c = threadIdx.x, H = C / 8;
   float* s_h = s_f + C;
@@ -763,7 +744,6 @@ __global__ void k_se_gate(const double* __restrict__ ssum, int stat_stride, cons
 }
 // y = x * gate[b][c] on channel-major data [B][C][V];  also plain swish when gate == nullptr
 __global__ void k_scale_or_swish(const float* __restrict__ x, const float* __restrict__ gate, float* __restrict__ y, size_t V, size_t total) {
-  pdl_prologue();
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   float v = x[i];
@@ -772,7 +752,6 @@ __global__ void k_scale_or_swish(const float* __restrict__ x, const float* __res
 
 // copy groups of a PF into another PF at a group offset (channel concatenation)
 __global__ void k_copy_groups(const float4* __restrict__ src, float4* __restrict__ dst, int Gs, int Gd, int g_off, int R) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R) return;
@@ -781,7 +760,6 @@ __global__ void k_copy_groups(const float4* __restrict__ src, float4* __restrict
 
 // broadcast a per-shape vector v[b][4*Gv] over all rows (the time embedding "expand")
 __global__ void k_fill_groups(const float* __restrict__ v, int v_stride, float4* __restrict__ dst, int Gd, int g_off, int R) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R) return;
@@ -795,7 +773,6 @@ __global__ void k_fill_groups(const float* __restrict__ v, int v_stride, float4*
 __global__ void k_devox_fuse(const float4* __restrict__ raw, const float4* __restrict__ nc, const float* __restrict__ scale,
                              const float* __restrict__ shift, const float4* __restrict__ rawp, AffSrc aff_p,
                              float4* __restrict__ out, int G, int C, int N, int r, int P, int Gd, int g_off) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   float4 sp = make_float4(0.f, 0.f, 0.f, 0.f), tp = sp;
@@ -826,7 +803,6 @@ __global__ void k_devox_fuse(const float4* __restrict__ raw, const float4* __res
 template <int A, int C, bool FULL>
 __global__ void __launch_bounds__(FPS_THREADS)
 k_fps_c4(const float4* __restrict__ c4, int* __restrict__ idx, float4* __restrict__ centers, int N, int M, int VT) {
-  pdl_prologue();
   extern __shared__ float s_fps[];
   int b = blockIdx.x;
   const float4* c = c4 + (size_t)b * N;
@@ -839,7 +815,6 @@ k_fps_c4(const float4* __restrict__ c4, int* __restrict__ idx, float4* __restric
 
 __global__ void k_ball_query_c4(const float4* __restrict__ centers, const float4* __restrict__ points, int* __restrict__ out,
                                 int N, int M, float r2, int K) {
-  pdl_prologue();
   int b = blockIdx.y;
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (warp >= M) return;
@@ -854,7 +829,6 @@ __global__ void k_ball_query_c4(const float4* __restrict__ centers, const float4
 __global__ void k_group_gather(const float4* __restrict__ feat, const float4* __restrict__ points,
                                const float4* __restrict__ centers, const int* __restrict__ nidx, float4* __restrict__ out,
                                int Gf, int N, int M, int U) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;    // g == 0: coordinates; g >= 1: features group g-1
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   int MU = M * U;
@@ -875,7 +849,6 @@ __global__ void k_group_gather(const float4* __restrict__ feat, const float4* __
 // ------------------------------------------------------------------------------------
 __global__ void k_three_nn_c4(const float4* __restrict__ points, const float4* __restrict__ centers, int* __restrict__ idx,
                               float* __restrict__ wgt, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   extern __shared__ float4 s_c4[];
@@ -905,7 +878,6 @@ __global__ void k_three_nn_c4(const float4* __restrict__ points, const float4* _
 
 __global__ void k_interp_rows(const float4* __restrict__ cf, const int* __restrict__ idx, const float* __restrict__ wgt,
                               float4* __restrict__ dst, int Gs, int M, int N, int Gd, int g_off) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= N) return;
@@ -929,7 +901,6 @@ constexpr int ATTN_CHUNK = 128;
 constexpr int ATTN_PART = 1024 + 64;
 __global__ void __launch_bounds__(256)
 k_attn_ctx(const float4* __restrict__ qkv, float* __restrict__ part, int H, int N) {
-  pdl_prologue();
   const int h = blockIdx.x, b = blockIdx.y, c = blockIdx.z, S = gridDim.z;
   const int Gq = 3 * H * 8;                       // groups in qkv
   const int n0 = c * ATTN_CHUNK, nn = min(ATTN_CHUNK, N - n0);
@@ -977,7 +948,6 @@ k_attn_ctx(const float4* __restrict__ qkv, float* __restrict__ part, int H, int 
 
 __global__ void __launch_bounds__(128)
 k_attn_apply(const float4* __restrict__ qkv, const float* __restrict__ part, float4* __restrict__ out, int H, int N, int S) {
-  pdl_prologue();
   int h = blockIdx.y, b = blockIdx.z;
   __shared__ float s_ctx[32 * 32];
   __shared__ float s_w[32][33];          // [chunk (<= 32)][d]: exp(max_c - max) / denominator
@@ -1026,7 +996,6 @@ k_attn_apply(const float4* __restrict__ qkv, const float* __restrict__ part, flo
 // layout conversion at the module-level C ABI: [B][C][R] channel-major <-> PF
 // ------------------------------------------------------------------------------------
 __global__ void k_cm_to_pf(const float* __restrict__ src, float4* __restrict__ dst, int C, int G, int R) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R) return;
@@ -1039,7 +1008,6 @@ __global__ void k_cm_to_pf(const float* __restrict__ src, float4* __restrict__ d
   dst[((size_t)b * G + g) * R + i] = make_float4(v[0], v[1], v[2], v[3]);
 }
 __global__ void k_pf_to_cm(const float4* __restrict__ src, float* __restrict__ dst, int C, int G, int R) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= R) return;
@@ -1054,7 +1022,6 @@ __global__ void k_pf_to_cm(const float4* __restrict__ src, float* __restrict__ d
 // dense voxel tensor [B][C][r^3] (flat index x*r^2 + y*r + z) <-> zero-haloed VG [B][G][(r+2)^3][4];
 // the halo rows of the VG must already be zero.  tf32 != 0: round to TF32 (rna) for the tensor cores.
 __global__ void k_cm_to_vg(const float* __restrict__ src, float4* __restrict__ dst, int C, int G, int r, int tf32) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   int V = r * r * r, rp = r + 2;
@@ -1072,7 +1039,6 @@ __global__ void k_cm_to_vg(const float* __restrict__ src, float4* __restrict__ d
   dst[((size_t)b * G + g) * ((size_t)rp * rp * rp) + prow] = o;
 }
 __global__ void k_vg_to_cm(const float4* __restrict__ src, float* __restrict__ dst, int C, int G, int r) {
-  pdl_prologue();
   int b = blockIdx.z, g = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   int V = r * r * r, rp = r + 2;
@@ -1088,7 +1054,6 @@ __global__ void k_vg_to_cm(const float4* __restrict__ src, float* __restrict__ d
   }
 }
 __global__ void k_cm_to_c4(const float* __restrict__ src, float4* __restrict__ dst, int N) {
-  pdl_prologue();
   int b = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -1096,7 +1061,6 @@ __global__ void k_cm_to_c4(const float* __restrict__ src, float4* __restrict__ d
   dst[(size_t)b * N + i] = make_float4(s[i], s[i + N], s[i + 2 * N], 0.0f);
 }
 __global__ void k_c4_to_cm(const float4* __restrict__ src, float* __restrict__ dst, int N) {
-  pdl_prologue();
   int b = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;

@@ -21,7 +21,6 @@ namespace lion {
 // ------------------------------------------------------------------------------------
 __global__ void k_grid_stats(const int* __restrict__ coords, int* __restrict__ ind, int* __restrict__ cnt,
                              int N, int r) {
-  pdl_prologue();
   int b = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -34,7 +33,6 @@ __global__ void k_grid_stats(const int* __restrict__ coords, int* __restrict__ i
 // one thread per (channel, point): coalesced feature reads, scattered atomics
 __global__ void k_avg_voxelize(const float* __restrict__ feat, const int* __restrict__ ind,
                                const int* __restrict__ cnt, float* __restrict__ out, int C, int N, int r3) {
-  pdl_prologue();
   int b = blockIdx.z;
   int c = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -53,7 +51,6 @@ __global__ void k_avg_voxelize(const float* __restrict__ feat, const int* __rest
 __global__ void k_trilinear_devox(const float* __restrict__ coords, const float* __restrict__ feat,
                                   int* __restrict__ inds, float* __restrict__ wgts, float* __restrict__ outs,
                                   int C, int N, int r, int is_training, int c_per_block) {
-  pdl_prologue();
   int b = blockIdx.z;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -87,7 +84,6 @@ __global__ void k_trilinear_devox(const float* __restrict__ coords, const float*
 template <int A, int C, bool FULL>
 __global__ void __launch_bounds__(FPS_THREADS)
 k_fps_soa(const float* __restrict__ coords, int* __restrict__ idx_out, int N, int M, int VT) {
-  pdl_prologue();
   extern __shared__ float s_fps[];
   int b = blockIdx.x;
   const float* c = coords + (size_t)b * 3 * N;
@@ -98,7 +94,6 @@ k_fps_soa(const float* __restrict__ coords, int* __restrict__ idx_out, int N, in
 
 __global__ void k_gather(const float* __restrict__ feat, const int* __restrict__ idx, float* __restrict__ out,
                          int C, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= M) return;
@@ -110,7 +105,6 @@ __global__ void k_gather(const float* __restrict__ feat, const int* __restrict__
 // ------------------------------------------------------------------------------------
 __global__ void k_ball_query_soa(const float* __restrict__ centers, const float* __restrict__ points,
                                  int* __restrict__ out, int N, int M, float r2, int K) {
-  pdl_prologue();
   int b = blockIdx.y;
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (warp >= M) return;
@@ -123,7 +117,6 @@ __global__ void k_ball_query_soa(const float* __restrict__ centers, const float*
 
 __global__ void k_grouping(const float* __restrict__ feat, const int* __restrict__ idx, float* __restrict__ out,
                            int C, int N, int MU) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= MU) return;
@@ -135,7 +128,6 @@ __global__ void k_grouping(const float* __restrict__ feat, const int* __restrict
 // ------------------------------------------------------------------------------------
 __global__ void k_three_nn_soa(const float* __restrict__ points, const float* __restrict__ centers,
                                int* __restrict__ idx, float* __restrict__ wgt, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   extern __shared__ float s_c[];   // [3][tile]
@@ -165,7 +157,6 @@ __global__ void k_three_nn_soa(const float* __restrict__ points, const float* __
 
 __global__ void k_three_interp(const float* __restrict__ cf, const int* __restrict__ idx,
                                const float* __restrict__ wgt, float* __restrict__ out, int C, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= N) return;
@@ -180,7 +171,6 @@ __global__ void k_three_interp(const float* __restrict__ cf, const int* __restri
 __global__ void __launch_bounds__(VOX_THREADS)
 k_voxel_coords_soa(const float* __restrict__ coords, float* __restrict__ norm_coords, int* __restrict__ vox,
                    int N, int r, int normalize, float eps) {
-  pdl_prologue();
   int b = blockIdx.x;
   const float* c = coords + (size_t)b * 3 * N;
   __shared__ float s_stat[4];
@@ -208,7 +198,6 @@ k_voxel_coords_soa(const float* __restrict__ coords, float* __restrict__ norm_co
 // avg_voxelize backward is a pure gather: grad_x[b][c][i] = grad_y[b][c][ind[i]] * (1 / cnt[ind[i]])
 __global__ void k_avg_voxelize_bwd(const float* __restrict__ gy, const int* __restrict__ ind, const int* __restrict__ cnt,
                                    float* __restrict__ gx, int C, int N, int r3) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -221,7 +210,6 @@ __global__ void k_avg_voxelize_bwd(const float* __restrict__ gy, const int* __re
 // trilinear devoxelize backward: 8 weighted scatter-adds per (point, channel) into the (pre-zeroed) grid gradient
 __global__ void k_trilinear_devox_bwd(const float* __restrict__ gy, const int* __restrict__ inds, const float* __restrict__ wgts,
                                       float* __restrict__ gx, int C, int N, int r3) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
@@ -234,7 +222,6 @@ __global__ void k_trilinear_devox_bwd(const float* __restrict__ gy, const int* _
 }
 // grouping backward: grad_x[b][c][idx[b][j][k]] += grad_y[b][c][j][k]
 __global__ void k_grouping_bwd(const float* __restrict__ gy, const int* __restrict__ idx, float* __restrict__ gx, int C, int N, int MU) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= MU) return;
@@ -243,7 +230,6 @@ __global__ void k_grouping_bwd(const float* __restrict__ gy, const int* __restri
 // 3-NN interpolation backward: grad_cf[b][c][idx_k[j]] += grad_y[b][c][j] * w_k[j], k = 0..2
 __global__ void k_three_interp_bwd(const float* __restrict__ gy, const int* __restrict__ idx, const float* __restrict__ wgt,
                                    float* __restrict__ gx, int C, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= N) return;
@@ -256,7 +242,6 @@ __global__ void k_three_interp_bwd(const float* __restrict__ gy, const int* __re
 }
 // gather backward: grad_x[b][c][idx[b][j]] += grad_y[b][c][j]
 __global__ void k_gather_bwd(const float* __restrict__ gy, const int* __restrict__ idx, float* __restrict__ gx, int C, int N, int M) {
-  pdl_prologue();
   int b = blockIdx.z, c = blockIdx.y;
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= M) return;

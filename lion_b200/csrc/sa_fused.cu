@@ -15,7 +15,6 @@
 #include "common.cuh"
 #include "model.cuh"
 #include "wgmma.cuh"
-#include <cstdlib>
 
 namespace lion {
 namespace saf {
@@ -205,9 +204,7 @@ constexpr size_t smem_bytes() {
 
 // shapes this file is instantiated for: (feature channels, layer-1 width, layer-2 width)
 bool sa_fused_usable(const SABlk& s) {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("LION_SA_FUSED"); on = e ? atoi(e) : 1; }
-  if (!on || s.mlp.conv.size() != 2 || s.k != 32 || s.m % 4) return false;
+  if (s.mlp.conv.size() != 2 || s.k != 32 || s.m % 4) return false;
   const ConvW &c1 = s.mlp.conv[0], &c2 = s.mlp.conv[1];
   if (!c1.tc.w || !c2.tc.w || c1.cout != c1.cout_pad || c2.cout != c2.cout_pad) return false;
   return s.cfeat == 32 && c1.cout == 32 && c2.cout == 64 && c1.tc.n == 32 && c2.tc.n == 64 && c1.tc.ck == 32 && c2.tc.ck == 32;
@@ -217,7 +214,6 @@ bool sa_fused_usable(const SABlk& s) {
 int sa_fused_run(Ctx* c, const SABlk& s, const float4* feat, const float4* points, const float4* centers, const int* nidx,
                  const float* scale1, const float* shift1, double* ssum, double* ssq, int stat_stride, float* pool_mm,
                  int B, int N) {
-  if (c->dry) return 0;
   saf::Params P{};
   const ConvW &c1 = s.mlp.conv[0], &c2 = s.mlp.conv[1];
   P.feat = feat; P.points = points; P.centers = centers; P.nidx = nidx;
@@ -236,9 +232,8 @@ int sa_fused_run(Ctx* c, const SABlk& s, const float4* feat, const float4* point
     LION_CHECK_CUDA(cudaFuncSetAttribute(saf::k_sa_fused<8, 32, 64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     LION_CHECK_CUDA(cudaFuncSetAttribute(saf::k_sa_fused<8, 32, 64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  if (!scale1) saf::k_sa_fused<8, 32, 64, 1><<<grid, 128, smem, c->stream>>>(P);
-  else saf::k_sa_fused<8, 32, 64, 2><<<grid, 128, smem, c->stream>>>(P);
-  c->launches++;
+  if (!scale1) LION_LAUNCH(c, (saf::k_sa_fused<8, 32, 64, 1>), grid, 128, smem, P);
+  else LION_LAUNCH(c, (saf::k_sa_fused<8, 32, 64, 2>), grid, 128, smem, P);
   return check_launch(c, "sa_fused");
 }
 

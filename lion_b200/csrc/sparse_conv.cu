@@ -117,7 +117,6 @@ bool ygemm_usable(const ConvW& y) {
 
 // y[b][v][0..ld) = x[b][v][:] * Wy for the first nocc[b] rows of every shape
 int ygemm_run(Ctx* c, const ConvW& y, const float4* xc, float* out, int ld, const int* nocc, int B, int N) {
-  if (c->dry) return 0;
   if (ld % 32) { set_error("ygemm: row pitch %d is not a multiple of 32", ld); return LION_ERR_ARG; }
   spc::Params P{};
   P.x = xc; P.w = y.tc.w; P.y = out; P.nocc = nocc;
@@ -137,8 +136,7 @@ int ygemm_run(Ctx* c, const ConvW& y, const float4* xc, float* out, int ld, cons
     LION_CHECK_CUDA(cudaFuncSetAttribute(spc::k_ygemm, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   }
   if (smem > 200 * 1024) { set_error("ygemm: %d input channels do not fit shared memory", y.cin_pad); return LION_ERR_ARG; }   // > 113 KB: one CTA per SM
-  spc::k_ygemm<<<dim3(n_tiles, slices), 256, smem, c->stream>>>(P);
-  c->launches++;
+  LION_LAUNCH(c, spc::k_ygemm, dim3(n_tiles, slices), 256, smem, P);
   return check_launch(c, "ygemm");
 }
 

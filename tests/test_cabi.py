@@ -123,8 +123,8 @@ def test_vae_state_dict_loads_strict():
 
 def test_shipped_library_contains_hopper_tensor_and_bulk_copy_sass():
     """The built liblion_b200.so must carry the sm_90a-native instructions the design rests on -- wgmma (HGMMA),
-    cp.async.bulk (UBLKCP), mbarriers (SYNCS) -- so that a silent fallback to the SIMT convolution
-    (`LION_CONV_IMPL=simt` is a debugging knob, not a build mode) cannot ship.  cuobjdump needs no GPU."""
+    cp.async.bulk (UBLKCP), mbarriers (SYNCS) -- so that a build whose convolutions all fall back to the SIMT kernel
+    (which only serves output widths that are not a multiple of 32) cannot ship.  cuobjdump needs no GPU."""
     import shutil
     import subprocess
     if shutil.which("cuobjdump") is None:

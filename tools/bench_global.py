@@ -30,6 +30,6 @@ for _ in range(n): g.replay()
 e1.record(); torch.cuda.synchronize()
 graph_us = e0.elapsed_time(e1) * 1000 / n
 print(json.dumps({"global_prior_forward_us_eager": eager_us, "global_prior_forward_us_graph": graph_us, "B": B,
-                  "launches_per_forward": L.last_launches(), "LION_GP_PERSIST": os.environ.get("LION_GP_PERSIST", "1"),
+                  "launches_per_forward": L.last_launches(),
                   "weights_mb": sum(p.numel() for p in m.parameters()) * 4 / 1e6,
                   "hbm_gbs_graph": sum(p.numel() for p in m.parameters()) * 4 / 1e3 / graph_us}))

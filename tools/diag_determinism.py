@@ -12,7 +12,7 @@ m = PVCNN2Prior(cfg.sde, 1, cfg); m.load_state_dict(synth_state_dict(keys['prior
 x, style = gen(31, 3, 8192, 1, 1).cuda(), gen(32, 3, 128, 1, 1).cuda()
 t = torch.tensor([1000.0, 500.0, 1.0]).cuda()
 a = m(x=x, t=t, condition_input=style); b = m(x=x, t=t, condition_input=style)
-print("impl", os.environ.get("LION_CONV_IMPL", "tc"), "same-call repeat: bitwise", torch.equal(a, b), "rel", rel_err(a, b))
+print("same-call repeat: bitwise", torch.equal(a, b), "rel", rel_err(a, b))
 one = m(x=x[1:2], t=t[1:2], condition_input=style[1:2])
 print("  B=3 vs B=1 rel", rel_err(one, a[1:2]))
 for (cin, cout, r, N) in [(64, 64, 32, 2048), (128, 128, 8, 64), (4, 32, 32, 2048)]:
