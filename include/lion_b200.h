@@ -222,6 +222,17 @@ int lion_chamfer_forward(const float* xyz1, const float* xyz2, float* dist1, flo
 int lion_chamfer_pairwise(const float* samples, const float* refs, float* out, int n_sample, int n_ref, int N, int M,
                           void* stream);
 
+/* Backward of lion_chamfer_forward (replaces chamfer_3D.backward, chamfer3D.cu:155-195): given the forward's
+ * idx1 / idx2 and the incoming graddist1 [B,N], graddist2 [B,M], writes (does not accumulate into)
+ *   gradxyz1[i] = g_i (xyz1_i - xyz2_idx1[i])  + sum over j with idx2[j] == i, ascending, of -(g'_j (xyz2_j - xyz1_i))
+ *   gradxyz2[j] = sum over i with idx1[i] == j, ascending, of -(g_i (xyz1_i - xyz2_j))  + g'_j (xyz2_j - xyz1_idx2[j])
+ * with g = 2 graddist1, g' = 2 graddist2, every product and sum rounded separately.  No atomics: the result is
+ * bit-reproducible, and an element with at most one scattered term equals the reference's bit for bit (the
+ * reference's fp32 atomicAdd order, and so its result, varies from run to run).  At most 65535 pairs per call. */
+int lion_chamfer_backward(const float* xyz1, const float* xyz2, const int* idx1, const int* idx2,
+                          const float* graddist1, const float* graddist2, float* gradxyz1, float* gradxyz2,
+                          int B, int N, int M, void* stream);
+
 /* Approximate earth mover's distance (third_party/PyTorchEMD/cuda/emd_kernel.cu:23-170 approxmatch +
  * :196-246 matchcost, as driven by emd_nograd.py:9-45): xyz1 [B,N,3], xyz2 [B,M,3] -> cost [B]
  * = sum_{k,l} |xyz1_k - xyz2_l|^2 * match[l][k] (NOT yet divided by N; the Python wrapper does that).
@@ -231,6 +242,19 @@ int lion_chamfer_pairwise(const float* samples, const float* refs, float* out, i
 int lion_emd_approx(const float* xyz1, const float* xyz2, float* cost, int B, int N, int M, void* stream);
 int lion_emd_pairwise(const float* samples, const float* refs, float* out, int n_sample, int n_ref, int N, int M,
                       void* stream);
+
+/* Differentiable approximate EMD (emd.py:6-24 EarthMoverDistanceFunction; emd_kernel.cu:280-396 matchcostgrad1/2).
+ * lion_emd_approx_saved computes the same cost as lion_emd_approx, bit for bit, and also writes the capacity ratios of
+ * every annealing level t = 0..9 (level -4^(7-t), the last 0): ratios [B][10][N+M], ratioL_t in [b][t][0..N),
+ * ratioR_t in [b][t][N..N+M) -- 40 (N+M) bytes per pair instead of the reference's 4 N M byte match matrix.
+ * lion_emd_backward rebuilds match[l][k] = sum_t exp(level_t |xyz1_k - xyz2_l|^2) ratioL_t[k] ratioR_t[l] from them on
+ * the fly (never in memory) and writes
+ *   grad1[k] = grad_cost[b] * sum_l 2 match[l][k] (xyz1_k - xyz2_l),   grad2[l] = grad_cost[b] * sum_k 2 match[l][k] (xyz2_l - xyz1_k)
+ * treating match as a constant, as the reference does.  Sums run in a fixed order: bit-reproducible.  N, M <= 2048. */
+int lion_emd_approx_saved(const float* xyz1, const float* xyz2, float* cost, float* ratios,
+                          int B, int N, int M, void* stream);
+int lion_emd_backward(const float* xyz1, const float* xyz2, const float* ratios, const float* grad_cost,
+                      float* grad1, float* grad2, int B, int N, int M, void* stream);
 
 /* measurement hook (bench.py roofline leg): average device time of `iters` launches of the
  * convolution kernel alone (CUDA events on `stream`), on synthetic data: ntaps = 27 -> 3x3x3

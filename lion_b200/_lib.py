@@ -75,7 +75,10 @@ def _proto(lib):
         "lion_scheduler_step": (P(vp, vp, vp, vp, vp, vp, sz, vp), i),
         "lion_chamfer_forward": (P(vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_chamfer_pairwise": (P(vp, vp, vp, i, i, i, i, vp), i),
+        "lion_chamfer_backward": (P(vp, vp, vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_emd_approx": (P(vp, vp, vp, i, i, i, vp), i),
+        "lion_emd_approx_saved": (P(vp, vp, vp, vp, i, i, i, vp), i),
+        "lion_emd_backward": (P(vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_emd_pairwise": (P(vp, vp, vp, i, i, i, i, vp), i),
         "lion_bench_conv": (P(vp, i, i, i, i, i, i, i, C.POINTER(f), C.POINTER(C.c_double), vp), i),
     }

@@ -188,9 +188,15 @@ __device__ __forceinline__ float emd_d2(float x1, float y1, float z1, float x2, 
   return (x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1) + (z2 - z1) * (z2 - z1);
 }
 
+constexpr int EMD_LEVELS = 10;                // annealing levels -4^7 .. -4^-1, 0
+
 // pair p: xyz1 = a[(p / nb) or p], xyz2 = b[(p % nb) or p]
+// SAVE: also write level t's ratioL to ratios[p][t][0..n) and its ratioR to ratios[p][t][n..n+m) -- all that
+// k_emd_backward needs to rebuild match[l][k] = sum_t exp(level_t d2(k,l)) ratioL_t[k] ratioR_t[l].
+template <bool SAVE>
 __global__ void __launch_bounds__(EMD_THREADS)
-k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* __restrict__ out, int n, int m, int nb, int pairwise) {
+k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* __restrict__ out, float* __restrict__ ratios,
+             int n, int m, int nb, int pairwise) {
   extern __shared__ float sm[];
   float4* p1 = reinterpret_cast<float4*>(sm);            // [n] x,y,z of xyz1 + ratioL
   float4* p2 = p1 + EMD_MAX;                             // [m] x,y,z of xyz2 + (remainR | ratioR)
@@ -210,6 +216,7 @@ k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* _
   for (int j = 7; j >= -2; j--) {
     float level = -powf(4.0f, j);
     if (j == -2) level = 0;
+    float* saved = SAVE ? ratios + ((size_t)p * EMD_LEVELS + (7 - j)) * (n + m) : nullptr;
     // ---- pass 1: ratioL[k] = remainL[k] / (1e-9 + sum_l exp(level d) remainR[l]) ---------------
     for (int l = tid; l < m; l += EMD_THREADS) p2[l].w = remainR[l];
     __syncthreads();
@@ -234,7 +241,10 @@ k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* _
 #pragma unroll
       for (int u = 0; u < EMD_Q; ++u) {
         int k = u * EMD_THREADS + tid;
-        if (k < n) p1[k].w = remainL[k] / suml[u];       // ratioL
+        if (k < n) {
+          p1[k].w = remainL[k] / suml[u];                // ratioL
+          if (SAVE) saved[k] = p1[k].w;
+        }
       }
     }
     __syncthreads();
@@ -263,6 +273,7 @@ k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* _
           float s = sumr[u] * r;
           float consumption = fminf(r / (s + 1e-9f), 1.0f);
           ratioR[l] = consumption * r;
+          if (SAVE) saved[n + l] = consumption * r;
           remainR[l] = fmaxf(0.0f, r - s);
         }
       }
@@ -309,24 +320,217 @@ k_emd_approx(const float* __restrict__ a, const float* __restrict__ bb, float* _
   }
 }
 
+// ---- backward (reference: emd_kernel.cu:280-353, matchcostgrad1 / matchcostgrad2) ---------------------------
+//   grad1[k] = gc * sum_l 2 match[l][k] (xyz1_k - xyz2_l),   grad2[l] = gc * sum_k 2 match[l][k] (xyz2_l - xyz1_k)
+// with match treated as a constant (the annealing is not differentiated), as in the reference.  match is rebuilt on
+// the fly from the ratios k_emd_approx<true> saved, with the forward's d2 and w expressions summed over the levels in
+// the forward's order, so it is never written to memory.  One CTA owns EMDB_ROWS rows of one direction of one pair;
+// each thread keeps its EMDB_Q rows' coordinates and ten ratios in registers and walks the other cloud (coordinates
+// and ten ratio rows: 56 B per point, 112 KB at 2048 points -> two CTAs per SM) in shared memory in index order.
+// Every sum runs in a fixed order: the result is bit-reproducible.
+constexpr int EMDB_THREADS = 256;
+constexpr int EMDB_Q = 2;                     // rows per thread
+constexpr int EMDB_ROWS = EMDB_THREADS * EMDB_Q;
+
+__host__ __device__ constexpr size_t emdb_smem(int cols) { return (size_t)cols * (sizeof(float4) + EMD_LEVELS * sizeof(float)); }
+
+// grid (pairs, 2 directions, row blocks): direction 0 -> rows are points of xyz1 (grad1), 1 -> points of xyz2 (grad2)
+__global__ void __launch_bounds__(EMDB_THREADS, 2)
+k_emd_backward(const float* __restrict__ xyz1, const float* __restrict__ xyz2, const float* __restrict__ ratios,
+               const float* __restrict__ grad_cost, float* __restrict__ grad1, float* __restrict__ grad2, int n, int m) {
+  extern __shared__ float4 smb[];
+  __shared__ float slevel[EMD_LEVELS];
+  const int p = blockIdx.x, dir = blockIdx.y, tid = threadIdx.x;
+  const int nrow = dir ? m : n, ncol = dir ? n : m;
+  const int row0 = blockIdx.z * EMDB_ROWS;
+  if (row0 >= nrow) return;                              // the shorter direction needs fewer row blocks
+  const float* rows = dir ? xyz2 + (size_t)p * m * 3 : xyz1 + (size_t)p * n * 3;
+  const float* cols = dir ? xyz1 + (size_t)p * n * 3 : xyz2 + (size_t)p * m * 3;
+  const float* rat = ratios + (size_t)p * EMD_LEVELS * (n + m);
+  const int roff = dir ? n : 0, coff = dir ? 0 : n;     // ratioL_t at [t][0..n), ratioR_t at [t][n..n+m)
+  float4* cxyz = smb;                                    // [ncol]
+  float* crat = reinterpret_cast<float*>(cxyz + ncol);   // [EMD_LEVELS][ncol]
+  for (int c = tid; c < ncol; c += EMDB_THREADS) cxyz[c] = make_float4(cols[c * 3], cols[c * 3 + 1], cols[c * 3 + 2], 0.f);
+  for (int t = 0; t < EMD_LEVELS; ++t)
+    for (int c = tid; c < ncol; c += EMDB_THREADS) crat[t * ncol + c] = rat[(size_t)t * (n + m) + coff + c];
+  // the forward's levels, evaluated by the same (run-time) powf
+  if (tid < EMD_LEVELS) slevel[tid] = tid == EMD_LEVELS - 1 ? 0.0f : -powf(4.0f, 7 - tid);
+  float x[EMDB_Q], y[EMDB_Q], z[EMDB_Q], rr[EMDB_Q][EMD_LEVELS], gx[EMDB_Q], gy[EMDB_Q], gz[EMDB_Q];
+#pragma unroll
+  for (int u = 0; u < EMDB_Q; ++u) {
+    const int r = row0 + u * EMDB_THREADS + tid;
+    const bool ok = r < nrow;
+    x[u] = ok ? rows[r * 3] : 0.f; y[u] = ok ? rows[r * 3 + 1] : 0.f; z[u] = ok ? rows[r * 3 + 2] : 0.f;
+#pragma unroll
+    for (int t = 0; t < EMD_LEVELS; ++t) rr[u][t] = ok ? rat[(size_t)t * (n + m) + roff + r] : 0.f;
+    gx[u] = gy[u] = gz[u] = 0.0f;
+  }
+  __syncthreads();
+  float level[EMD_LEVELS];
+#pragma unroll
+  for (int t = 0; t < EMD_LEVELS; ++t) level[t] = slevel[t];
+  for (int c = 0; c < ncol; ++c) {
+    const float4 q = cxyz[c];
+    float cr[EMD_LEVELS];
+#pragma unroll
+    for (int t = 0; t < EMD_LEVELS; ++t) cr[t] = crat[t * ncol + c];
+#pragma unroll
+    for (int u = 0; u < EMDB_Q; ++u) {
+      // d2 and w exactly as k_emd_approx pass 3: emd_d2(xyz1_k, xyz2_l), exp(level d2) * ratioL_k * ratioR_l
+      const float d2 = dir ? emd_d2(q.x, q.y, q.z, x[u], y[u], z[u]) : emd_d2(x[u], y[u], z[u], q.x, q.y, q.z);
+      float match = 0.0f;
+#pragma unroll
+      for (int t = 0; t < EMD_LEVELS; ++t) {
+        const float w = dir ? __expf(level[t] * d2) * cr[t] * rr[u][t] : __expf(level[t] * d2) * rr[u][t] * cr[t];
+        match += w;
+      }
+      const float d = match * 2;
+      gx[u] += (x[u] - q.x) * d;
+      gy[u] += (y[u] - q.y) * d;
+      gz[u] += (z[u] - q.z) * d;
+    }
+  }
+  const float gc = grad_cost[p];
+  float* g = dir ? grad2 + (size_t)p * m * 3 : grad1 + (size_t)p * n * 3;
+#pragma unroll
+  for (int u = 0; u < EMDB_Q; ++u) {
+    const int r = row0 + u * EMDB_THREADS + tid;
+    if (r < nrow) { g[r * 3] = gx[u] * gc; g[r * 3 + 1] = gy[u] * gc; g[r * 3 + 2] = gz[u] * gc; }
+  }
+}
+
+// =====================================================================================
+// Chamfer backward (reference: chamfer3D.cu:155-195, NmDistanceGradKernel launched once per direction with fp32
+// atomicAdd scatters into zeroed gradients).  Here every output element is owned by one thread and written once:
+// for a point i of cloud 1
+//   grad1[i] = g_i (x1_i - x2_idx1[i])  then, in ascending j,  + (-(g'_j (x2_j - x1_i)))  for every j with idx2[j] == i
+// (g = 2 graddist1, g' = 2 graddist2); cloud 2 symmetrically, but its scattered terms first and its direct term last,
+// which is the reference's launch order.  The j are found by scanning the other cloud's index array, staged in shared
+// memory in chunks (integer compares only).  Products and sums are rounded one by one (no contraction), as the
+// reference's atomics do: an element with at most one scattered term equals the reference's result bit for bit, and
+// every element is bit-reproducible.
+// =====================================================================================
+constexpr int CDB_THREADS = 256;
+constexpr int CDB_CHUNK = 4096;               // other-cloud indices staged per pass (16 KB)
+
+__device__ __forceinline__ void cdb_add(float& sx, float& sy, float& sz, float g, float ax, float ay, float az, float bx,
+                                        float by, float bz, bool neg) {
+  float tx = __fmul_rn(g, __fsub_rn(ax, bx)), ty = __fmul_rn(g, __fsub_rn(ay, by)), tz = __fmul_rn(g, __fsub_rn(az, bz));
+  if (neg) { tx = -tx; ty = -ty; tz = -tz; }
+  sx = __fadd_rn(sx, tx); sy = __fadd_rn(sy, ty); sz = __fadd_rn(sz, tz);
+}
+
+// grid (cdiv(n, T) + cdiv(m, T), B): the first cdiv(n, T) blocks own points of xyz1, the rest points of xyz2
+__global__ void __launch_bounds__(CDB_THREADS)
+k_chamfer_backward(const float* __restrict__ xyz1, const float* __restrict__ xyz2, const int* __restrict__ idx1,
+                   const int* __restrict__ idx2, const float* __restrict__ gd1, const float* __restrict__ gd2,
+                   float* __restrict__ gx1, float* __restrict__ gx2, int n, int m) {
+  __shared__ int4 sidx[CDB_CHUNK / 4];
+  const size_t b = blockIdx.y;
+  const int nb1 = (n + CDB_THREADS - 1) / CDB_THREADS;
+  const bool two = (int)blockIdx.x >= nb1;              // rows are points of xyz2
+  const int na = two ? m : n, nb = two ? n : m;
+  const float* A = (two ? xyz2 : xyz1) + b * na * 3;
+  const float* Bp = (two ? xyz1 : xyz2) + b * nb * 3;
+  const int* ia = (two ? idx2 : idx1) + b * na;
+  const int* ib = (two ? idx1 : idx2) + b * nb;
+  const float* ga = (two ? gd2 : gd1) + b * na;
+  const float* gb = (two ? gd1 : gd2) + b * nb;
+  const int i = ((int)blockIdx.x - (two ? nb1 : 0)) * CDB_THREADS + threadIdx.x;
+  const bool valid = i < na;
+  float ax = 0.f, ay = 0.f, az = 0.f, sx = 0.f, sy = 0.f, sz = 0.f;
+  if (valid) {
+    ax = A[i * 3]; ay = A[i * 3 + 1]; az = A[i * 3 + 2];
+    if (!two) {                                        // cloud 1: direct term first
+      const int j = ia[i];
+      cdb_add(sx, sy, sz, ga[i] * 2, ax, ay, az, Bp[j * 3], Bp[j * 3 + 1], Bp[j * 3 + 2], false);
+    }
+  }
+  int* s = reinterpret_cast<int*>(sidx);
+  for (int c0 = 0; c0 < nb; c0 += CDB_CHUNK) {
+    const int cn = min(CDB_CHUNK, nb - c0), cn4 = (cn + 3) >> 2;
+    __syncthreads();
+    for (int k = threadIdx.x; k < cn4 * 4; k += CDB_THREADS) s[k] = k < cn ? ib[c0 + k] : -1;
+    __syncthreads();
+    if (!valid) continue;
+#pragma unroll 4
+    for (int k4 = 0; k4 < cn4; ++k4) {
+      const int4 v = sidx[k4];
+      if (v.x == i || v.y == i || v.z == i || v.w == i) {
+        const int e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          if (e[u] != i) continue;
+          const int j = c0 + k4 * 4 + u;
+          cdb_add(sx, sy, sz, gb[j] * 2, Bp[j * 3], Bp[j * 3 + 1], Bp[j * 3 + 2], ax, ay, az, true);
+        }
+      }
+    }
+  }
+  if (!valid) return;
+  if (two) {                                           // cloud 2: direct term last
+    const int j = ia[i];
+    cdb_add(sx, sy, sz, ga[i] * 2, ax, ay, az, Bp[j * 3], Bp[j * 3 + 1], Bp[j * 3 + 2], false);
+  }
+  float* out = (two ? gx2 : gx1) + b * na * 3;
+  out[i * 3] = sx; out[i * 3 + 1] = sy; out[i * 3 + 2] = sz;
+}
+
 }  // namespace lion
 
-static int emd_launch(const float* a, const float* b, float* out, int pairs, int n, int m, int nb, int pairwise, void* stream) {
+extern "C" int lion_chamfer_backward(const float* xyz1, const float* xyz2, const int* idx1, const int* idx2,
+                                     const float* graddist1, const float* graddist2, float* gradxyz1, float* gradxyz2,
+                                     int B, int N, int M, void* stream) {
+  LION_REQUIRE(xyz1 && xyz2 && idx1 && idx2 && graddist1 && graddist2 && gradxyz1 && gradxyz2 && B > 0 && N > 0 && M > 0,
+               "lion_chamfer_backward: bad arguments");
+  LION_REQUIRE(B <= 65535, "lion_chamfer_backward: at most 65535 cloud pairs per call (got %d)", B);
+  Ctx c;
+  c.stream = (cudaStream_t)stream;
+  LION_LAUNCH(&c, k_chamfer_backward, dim3(cdiv(N, CDB_THREADS) + cdiv(M, CDB_THREADS), B), CDB_THREADS, 0, xyz1, xyz2, idx1,
+              idx2, graddist1, graddist2, gradxyz1, gradxyz2, N, M);
+  return check_launch(&c, "lion_chamfer_backward");
+}
+
+template <bool SAVE>
+static int emd_launch(const float* a, const float* b, float* out, float* ratios, int pairs, int n, int m, int nb, int pairwise,
+                      void* stream) {
   Ctx c;
   c.stream = (cudaStream_t)stream;
   const size_t smem = (size_t)EMD_MAX * (2 * sizeof(float4) + 3 * sizeof(float)) + EMD_THREADS * sizeof(float);
   static DevOnce attr_once;
   if (attr_once.need()) {
-    LION_CHECK_CUDA(cudaFuncSetAttribute(k_emd_approx, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LION_CHECK_CUDA(cudaFuncSetAttribute(k_emd_approx<SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 }
-  LION_LAUNCH(&c, k_emd_approx, pairs, EMD_THREADS, smem, a, b, out, n, m, nb, pairwise);
-  return check_launch(&c, "lion_emd_approx");
+  LION_LAUNCH(&c, k_emd_approx<SAVE>, pairs, EMD_THREADS, smem, a, b, out, ratios, n, m, nb, pairwise);
+  return check_launch(&c, SAVE ? "lion_emd_approx_saved" : "lion_emd_approx");
 }
 
 extern "C" int lion_emd_approx(const float* xyz1, const float* xyz2, float* cost, int B, int N, int M, void* stream) {
   LION_REQUIRE(xyz1 && xyz2 && cost && B > 0 && N > 0 && M > 0, "lion_emd_approx: bad arguments");
   LION_REQUIRE(N <= EMD_MAX && M <= EMD_MAX, "lion_emd_approx: clouds of at most %d points (got %d, %d)", EMD_MAX, N, M);
-  return emd_launch(xyz1, xyz2, cost, B, N, M, 1, 0, stream);
+  return emd_launch<false>(xyz1, xyz2, cost, nullptr, B, N, M, 1, 0, stream);
+}
+
+extern "C" int lion_emd_approx_saved(const float* xyz1, const float* xyz2, float* cost, float* ratios, int B, int N, int M,
+                                     void* stream) {
+  LION_REQUIRE(xyz1 && xyz2 && cost && ratios && B > 0 && N > 0 && M > 0, "lion_emd_approx_saved: bad arguments");
+  LION_REQUIRE(N <= EMD_MAX && M <= EMD_MAX, "lion_emd_approx_saved: clouds of at most %d points (got %d, %d)", EMD_MAX, N, M);
+  return emd_launch<true>(xyz1, xyz2, cost, ratios, B, N, M, 1, 0, stream);
+}
+
+extern "C" int lion_emd_backward(const float* xyz1, const float* xyz2, const float* ratios, const float* grad_cost, float* grad1,
+                                 float* grad2, int B, int N, int M, void* stream) {
+  LION_REQUIRE(xyz1 && xyz2 && ratios && grad_cost && grad1 && grad2 && B > 0 && N > 0 && M > 0, "lion_emd_backward: bad arguments");
+  LION_REQUIRE(N <= EMD_MAX && M <= EMD_MAX, "lion_emd_backward: clouds of at most %d points (got %d, %d)", EMD_MAX, N, M);
+  Ctx c;
+  c.stream = (cudaStream_t)stream;
+  static DevOnce attr_once;
+  if (attr_once.need()) {
+    LION_CHECK_CUDA(cudaFuncSetAttribute(k_emd_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)emdb_smem(EMD_MAX)));
+  }
+  LION_LAUNCH(&c, k_emd_backward, dim3(B, 2, cdiv(N > M ? N : M, EMDB_ROWS)), EMDB_THREADS, emdb_smem(N > M ? N : M), xyz1, xyz2,
+              ratios, grad_cost, grad1, grad2, N, M);
+  return check_launch(&c, "lion_emd_backward");
 }
 
 extern "C" int lion_emd_pairwise(const float* samples, const float* refs, float* out, int n_sample, int n_ref, int N, int M,
@@ -334,5 +538,5 @@ extern "C" int lion_emd_pairwise(const float* samples, const float* refs, float*
   LION_REQUIRE(samples && refs && out && n_sample > 0 && n_ref > 0 && N > 0 && M > 0, "lion_emd_pairwise: bad arguments");
   LION_REQUIRE(N <= EMD_MAX && M <= EMD_MAX, "lion_emd_pairwise: clouds of at most %d points (got %d, %d)", EMD_MAX, N, M);
   LION_REQUIRE((long long)n_sample * n_ref < (1LL << 31), "lion_emd_pairwise: too many pairs");
-  return emd_launch(samples, refs, out, n_sample * n_ref, N, M, n_ref, 1, stream);
+  return emd_launch<false>(samples, refs, out, nullptr, n_sample * n_ref, N, M, n_ref, 1, stream);
 }

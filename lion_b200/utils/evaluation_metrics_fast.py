@@ -6,11 +6,17 @@ utils/evaluation_metrics_fast.py: `distChamferCUDAnograd` (:83-88 region) and th
 (lion_chamfer_pairwise: a CTA per (sample, reference) pair, both directions, means reduced on
 chip) instead of the reference's Python double loop with an expanded copy of the sample cloud
 per reference batch; metric='EMD' likewise (lion_emd_pairwise: the fused approxmatch + matchcost
-kernel per pair, no [Nr, M, N] match matrices)."""
+kernel per pair, no [Nr, M, N] match matrices).
+
+The reconstruction losses of utils/model_helper.py:17-74 are differentiable: `distChamferCUDA` (reference :99-109)
+and `emd_approx(require_grad=True)` (reference :122-147) backpropagate through the library's Chamfer and EMD
+backward kernels.  `distChamferCUDA_l1` (reference :31-57) is not provided: it imports `models.pvcnn.functional`,
+which does not exist in the reference tree."""
 import torch
 
 from .. import _lib as L
-from ..third_party.ChamferDistancePytorch.chamfer3D.dist_chamfer_3D import chamfer_3DDist_nograd
+from ..third_party.ChamferDistancePytorch.chamfer3D.dist_chamfer_3D import chamfer_3DDist, chamfer_3DDist_nograd
+from ..third_party.PyTorchEMD.emd import earth_mover_distance
 from ..third_party.PyTorchEMD.emd_nograd import earth_mover_distance_nograd
 
 
@@ -40,11 +46,18 @@ def pairwise_CD(sample_pcs, ref_pcs):
     return out
 
 
+def distChamferCUDA(x, y):
+    """x [B,N,3], y [B,M,3] -> (dist1 [B,N], dist2 [B,M]), differentiable (reference :99-109)."""
+    assert x.dim() == 3 and y.dim() == 3 and x.shape[2] == 3 and y.shape[2] == 3, f'get {x.shape} and {y.shape}'
+    dist1, dist2, _, _ = chamfer_3DDist()(x.cuda(), y.cuda())
+    return dist1, dist2
+
+
 def emd_approx(sample, ref, require_grad=True):
-    """[B,N,3] x [B,M,3] -> [B] approximate EMD / N (reference :122-147; forward only)."""
-    if require_grad and torch.is_grad_enabled() and (sample.requires_grad or ref.requires_grad):
-        raise NotImplementedError("lion_b200: the EMD backward kernel (training loss) is out of scope")
-    return earth_mover_distance_nograd(sample.cuda(), ref.cuda(), transpose=False)
+    """[B,N,3] x [B,M,3] -> [B] approximate EMD / N (reference :122-147); differentiable when require_grad."""
+    if not require_grad:
+        return earth_mover_distance_nograd(sample.cuda(), ref.cuda(), transpose=False)
+    return earth_mover_distance(sample.cuda(), ref.cuda(), transpose=False)
 
 
 @torch.no_grad()
