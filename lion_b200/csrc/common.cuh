@@ -55,11 +55,7 @@ struct Ctx {
   int num_sms = 132;
   int l2_bytes = 50 << 20;
   cudaStream_t stream = nullptr;
-  cudaStream_t aux = nullptr;     // side stream for work that is independent of the main chain (FPS)
-  cudaEvent_t ev_fork = nullptr;
-  cudaEvent_t ev_temb = nullptr;
-  cudaEvent_t ev_vox[4] = {nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaStream_t aux = nullptr;     // side stream for work that is independent of the main chain (FPS, neighbour searches)
   char* base = nullptr;      // arena
   char* zgrid = nullptr;     // persistent all-zero voxel grid (scatter target; re-zeroed after use)
   size_t zgrid_cap = 0, zgrid_need = 0;
@@ -111,10 +107,12 @@ static __global__ void k_stamp(unsigned long long* p) {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   *p = t;
 }
+// stamps on the side stream are named "aux:<name>"
 inline void stamp(Ctx* c, cudaStream_t s, const char* name, int idx = -1) {
   if (!c->d_stamps || c->dry || c->n_stamps >= LION_MAX_STAMPS) return;
-  if (idx >= 0) snprintf(c->stamp_names[c->n_stamps], 24, "%s%d", name, idx);
-  else snprintf(c->stamp_names[c->n_stamps], 24, "%s", name);
+  const char* pre = s == c->aux ? "aux:" : "";
+  if (idx >= 0) snprintf(c->stamp_names[c->n_stamps], 24, "%s%s%d", pre, name, idx);
+  else snprintf(c->stamp_names[c->n_stamps], 24, "%s%s", pre, name);
   k_stamp<<<1, 1, 0, s>>>(c->d_stamps + c->n_stamps);
   c->n_stamps++;
 }

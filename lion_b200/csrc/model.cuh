@@ -76,12 +76,20 @@ struct Block {
   int kind;   // LION_KIND_PVCONV / SA / FP
   PVConvBlk pv; SABlk sa; FPBlk fp;
 };
+// Point level l of the U-Net: the input points of SA level l, which FP stage n_sa - 1 - l interpolates back onto.
+// What the side stream prepares for it (unet_forward) is fixed by the architecture and decided at build time.
+struct UnetLevel {
+  std::vector<int> vox_r;   // distinct PVConv resolutions on these points: the SA level's first, then the FP stage's
+  cudaEvent_t sa_done = nullptr, vox_done = nullptr, nn_done = nullptr;   // FPS + ball query, voxel preps, 3-NN
+};
 struct UnetBlk {
   int num_classes, embed_dim, extra, input_dim, use_att, clip, clip_dim, S;
   const float *e0w = nullptr, *e0b = nullptr, *e2w = nullptr, *e2b = nullptr;
   const float *cfw = nullptr, *cfb = nullptr, *scw = nullptr, *scb = nullptr;
   float* d_freqs = nullptr;
   std::vector<std::vector<Block>> sa, fp;
+  std::vector<UnetLevel> levels;                          // [n_sa]
+  cudaEvent_t aux_start = nullptr, temb_done = nullptr;   // the side stream may start; the time embedding is done
   AttnBlk gatt;
   SharedMLPBlk cls0;
   ConvW cls2;
@@ -105,6 +113,7 @@ struct Model {
   std::vector<int> desc;
   std::vector<const float*> params;
   std::vector<void*> owned;
+  std::vector<cudaEvent_t> events;
   std::vector<PackJob> jobs;
   std::vector<StyleLayer> style_layers;
   StyleLayer* d_style_layers = nullptr;
@@ -129,8 +138,15 @@ struct Model {
     *p = (T*)q;
     return 0;
   }
+  int make_event(cudaEvent_t* e) {
+    cudaError_t r = cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+    if (r != cudaSuccess) { set_error("cudaEventCreate failed: %s", cudaGetErrorString(r)); return LION_ERR_CUDA; }
+    events.push_back(*e);
+    return 0;
+  }
   ~Model() {
     for (void* q : owned) cudaFree(q);
+    for (cudaEvent_t e : events) cudaEventDestroy(e);
     if (aff_cache) cudaFree(aff_cache);
     if (gp) global_prior_free(gp);
   }

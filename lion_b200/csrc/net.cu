@@ -17,6 +17,8 @@
 //   * voxel indices, counts and normalised coordinates are computed once per distinct
 //     (coords, resolution) -- 4x per step instead of 14x;
 //   * no permutes: the latent [B,N,4] is already a packed-feature tensor.
+#include <algorithm>
+#include <deque>
 #include <memory>
 #include <cstdlib>
 #include <cmath>
@@ -250,7 +252,19 @@ struct Fwd {
   char* stat_pool = nullptr;     // all GroupNorm statistics of a forward: zeroed by ONE memset
   size_t stat_off = 0, stat_cap = 0;
   float* aff = nullptr;          // [B][style_total] all AdaGN (factor|bias) vectors of this forward
-  std::vector<VoxPrep> vox;
+  std::deque<VoxPrep> vox;       // a deque: get_vox hands out pointers that later preps must not move
+};
+// One point level of a forward: SA level i's input points, the centres its FPS samples from them (the points of
+// level i + 1) with their ball-query neighbours, and the 3-NN of the points among the centres that the FP stage
+// interpolating back onto them uses.  An event is set from the side stream's record of the result until the main
+// stream has waited for it (wait_once).
+struct Level {
+  const float4* pts = nullptr; int n = 0;
+  PF feat;                                        // features at pts (the FP stage's skip input)
+  float4* centers = nullptr; int m = 0;
+  int* nidx = nullptr;                            // [B][m][k]
+  int* nn_idx = nullptr; float* nn_wgt = nullptr;  // [B][n][3]
+  cudaEvent_t sa_done = nullptr, vox_done = nullptr, nn_done = nullptr;   // centres + nidx, voxel preps of pts, nn_*
 };
 
 static PF alloc_pf(Fwd& f, int G, int R) {
@@ -356,10 +370,10 @@ static int alloc_stats(Fwd& f, int stride, double** ssum, double** ssq) {
 }
 
 // convolution + GroupNorm statistics (epilogue) + AdaGN(/SE) fold (k_affine_prep).
-// Round 2 tried computing the fold in the LAST CTA of the convolution (arrival ticket, no extra launch): measured
-// 1.3-2.0 ms per step SLOWER at B = 32 (profiles/r02_affine_fold_ab.json) -- a single SM folding 2048-4096 (b, c) pairs
-// with cold code on the critical path loses to a 32-CTA kernel whose launch latency the graph mostly hides -- so the
-// separate launch stays.
+// Computing the fold in the LAST CTA of the convolution instead (arrival ticket, no extra launch) measured 1.3-2.0 ms
+// per step SLOWER at B = 32 on the B200, before the port to H100 -- a single SM folding 2048-4096 (b, c) pairs with cold
+// code on the critical path loses to a 32-CTA kernel whose launch latency the graph mostly hides -- so the separate
+// launch stays.
 static int conv_gn(Fwd& f, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, const ConvGeom& geo,
                    const AdaGNW& g, double count, const float* se1, const float* se2, AffSrc& a) {
   double *ssum, *ssq;
@@ -537,9 +551,9 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   }
   LION_TRY(run_prep(f, j1, &jp));
   stamp(f.c, f.c->stream, " conv1");
-  // AdaGN-1 + Swish as a stand-alone pass over the grid (HBM-bound).  Round 2 tried to fold it into conv2's operand
-  // staging ("transform on load"): parity-green but 3.5x slower convolutions, deleted --
-  // profiles/r02_xf_transform_on_load_experiment.txt.  Its extra blocks re-zero the scatter grid (was: k_unscatter).
+  // AdaGN-1 + Swish as a stand-alone pass over the grid (HBM-bound).  Folding it into conv2's operand staging
+  // ("transform on load") was parity-green but made the convolutions 3.5x slower (measured on the B200, before the
+  // port to H100).  Its extra blocks re-zero the scatter grid (was: k_unscatter).
   float4* act1 = alloc_vg(f, Gout, r);
   {
     const int nb_act = cdiv(P, 256 * ACT_U);
@@ -595,39 +609,61 @@ static int fps_c4(Ctx* c, cudaStream_t s, int B, const float4* c4, int* fidx, fl
   return rc;
 }
 
-// SA module: (features PF, coords) -> (dst PF with Gd groups at g_off, centres C4)
-// pre_fps >= 0: the centres were already sampled on the side stream (event ev[pre_fps])
-static int sa_fwd(Fwd& f, const SABlk& s, PF feat, const float4* c4, float4* centers, float4* dst, int Gd, int g_off,
-                  int pre_fps = -1, const int* pre_nidx = nullptr) {
-  int N = feat.R, M = s.m, U = s.k, Gf = s.cfeat / 4;
-  if (feat.G != Gf) { set_error("SA: got %d feature channels, expected %d", feat.G * 4, s.cfeat); return LION_ERR_ARG; }
+// the side stream records `e` once its result is complete and leaves it in `slot`; the main stream waits for it
+// where it first needs the result, and only there
+static int record_on_aux(Ctx* c, cudaEvent_t e, cudaEvent_t& slot) {
+  if (!c->dry) { LION_CHECK_CUDA(cudaEventRecord(e, c->aux)); slot = e; }
+  return 0;
+}
+static int wait_once(Ctx* c, cudaEvent_t& slot) {
+  if (slot) LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, slot, 0));
+  slot = nullptr;
+  return 0;
+}
+
+// SA geometry of level i, on stream st: FPS of s.m centres out of lv.pts into lv.centers (allocated by the caller),
+// then the ball query of the k neighbours of each centre
+static int sa_geometry(Fwd& f, cudaStream_t st, const SABlk& s, Level& lv, int i) {
+  const int N = lv.n, M = s.m;
   if (N > FPS_MAX_N) { set_error("SA: N=%d too large for FPS", N); return LION_ERR_ARG; }
   if (M > N) { set_error("SA: more centres (%d) than points (%d)", M, N); return LION_ERR_ARG; }
+  lv.m = M;
+  int* fidx = f.c->alloc_n<int>((size_t)f.B * M);
+  LION_TRY(fps_c4(f.c, st, f.B, lv.pts, fidx, lv.centers, N, M));
+  stamp(f.c, st, "fps", i);
+  lv.nidx = f.c->alloc_n<int>((size_t)f.B * M * s.k);
+  LION_LAUNCH_ON(f.c, st, k_ball_query_c4, dim3(cdiv(M * 32, 256), f.B), 256, 0, lv.centers, lv.pts, lv.nidx, N, M,
+                 s.radius * s.radius, s.k);
+  stamp(f.c, st, "ballq", i);
+  return 0;
+}
+// FP geometry of level i, on stream st: the 3 nearest centres of every point and their interpolation weights
+static int fp_geometry(Fwd& f, cudaStream_t st, Level& lv, int i) {
+  lv.nn_idx = f.c->alloc_n<int>((size_t)f.B * lv.n * 3);
+  lv.nn_wgt = f.c->alloc_n<float>((size_t)f.B * lv.n * 3);
+  LION_LAUNCH_ON(f.c, st, k_three_nn_c4, dim3(cdiv(lv.n, 128), f.B), 128, 1024 * sizeof(float4), lv.pts, lv.centers, lv.nn_idx,
+                 lv.nn_wgt, lv.n, lv.m);
+  stamp(f.c, st, "3nn", i);
+  return 0;
+}
+
+// SA module: features PF at lv.pts -> dst PF (Gd groups at g_off) at lv.centers
+static int sa_fwd(Fwd& f, const SABlk& s, PF feat, Level& lv, float4* dst, int Gd, int g_off) {
+  int N = feat.R, M = s.m, U = s.k, Gf = s.cfeat / 4;
+  if (feat.G != Gf) { set_error("SA: got %d feature channels, expected %d", feat.G * 4, s.cfeat); return LION_ERR_ARG; }
   size_t mk = f.c->mark();
-  if (pre_fps >= 0) {
-    if (!f.c->dry) LION_CHECK_CUDA(cudaStreamWaitEvent(f.c->stream, f.c->ev[pre_fps], 0));
-  } else {
-    int* fidx = f.c->alloc_n<int>((size_t)f.B * M);
-    LION_TRY(fps_c4(f.c, f.c->stream, f.B, c4, fidx, centers, N, M));
-  }
-  const int* nidx = pre_nidx;                     // ball query already ran on the side stream (behind event ev[pre_fps])
-  if (!nidx) {
-    int* ni = f.c->alloc_n<int>((size_t)f.B * M * U);
-    float r2 = s.radius * s.radius;
-    LION_LAUNCH(f.c, k_ball_query_c4, dim3(cdiv(M * 32, 256), f.B), 256, 0, centers, c4, ni, N, M, r2, U);
-    nidx = ni;
-  }
+  LION_TRY(wait_once(f.c, lv.sa_done));
   if (sa_fused_usable(s)) {
     // gather -> conv -> AdaGN/Swish -> conv -> max-pool in two fused passes (sa_fused.cu): no [B, C, M, 32] round trips
     const ConvW &c1 = s.mlp.conv[0], &c2 = s.mlp.conv[1];
     double *s1, *q1, *s2, *q2;
     AffSrc a1, a2;
     LION_TRY(alloc_stats(f, c1.cout_pad, &s1, &q1));
-    LION_TRY(sa_fused_run(f.c, s, feat.p, c4, centers, nidx, nullptr, nullptr, s1, q1, c1.cout_pad, nullptr, f.B, N));
+    LION_TRY(sa_fused_run(f.c, s, feat.p, lv.pts, lv.centers, lv.nidx, nullptr, nullptr, s1, q1, c1.cout_pad, nullptr, f.B, N));
     LION_TRY(run_affine(f, s.mlp.gn[0], s1, q1, c1.cout_pad, (double)M * U, nullptr, nullptr, a1));
     LION_TRY(alloc_stats(f, c2.cout_pad, &s2, &q2));
     float* mm = f.c->alloc_n<float>((size_t)f.B * (c2.cout / 4) * M * 8);
-    LION_TRY(sa_fused_run(f.c, s, feat.p, c4, centers, nidx, a1.scale, a1.shift, s2, q2, c2.cout_pad, mm, f.B, N));
+    LION_TRY(sa_fused_run(f.c, s, feat.p, lv.pts, lv.centers, lv.nidx, a1.scale, a1.shift, s2, q2, c2.cout_pad, mm, f.B, N));
     LION_TRY(run_affine(f, s.mlp.gn[1], s2, q2, c2.cout_pad, (double)M * U, nullptr, nullptr, a2));
     LION_LAUNCH(f.c, k_act_pool_minmax, dim3(cdiv(M, 256), c2.cout / 4, f.B), 256, 0, (const float4*)mm, dst, a2, c2.cout / 4, c2.cout, M,
                 Gd, g_off);
@@ -636,36 +672,52 @@ static int sa_fwd(Fwd& f, const SABlk& s, PF feat, const float4* c4, float4* cen
     return 0;
   }
   PF grp = alloc_pf(f, Gf + 1, M * U);
-  LION_LAUNCH(f.c, k_group_gather, dim3(cdiv(M * U, 256), Gf + 1, f.B), 256, 0, feat.p, c4, centers, nidx, grp.p, Gf, N, M, U);
+  LION_LAUNCH(f.c, k_group_gather, dim3(cdiv(M * U, 256), Gf + 1, f.B), 256, 0, feat.p, lv.pts, lv.centers, lv.nidx, grp.p, Gf, N, M, U);
   LION_TRY(check_launch(f.c, "sa grouping"));
   LION_TRY(shared_mlp_fwd(f, s.mlp, grp, 32, dst, Gd, g_off));
   f.c->release(mk);
   return 0;
 }
 
-// FP module: interpolate centres' features to the points, concat skip, SharedMLP
-static int fp_fwd(Fwd& f, const FPBlk& b, const float4* pts_c4, int N, const float4* ctr_c4, int M, PF cfeat, PF skip,
-                  float4* dst, int Gd, int g_off, const int* pre_idx = nullptr, const float* pre_wgt = nullptr, int pre_ev = -1) {
-  int Gc = b.cc / 4, Gs = roundup(b.cp, 4) / 4;
+// FP module: interpolate the features at lv.centers (cfeat) to lv.pts, concat the skip features lv.feat, SharedMLP
+static int fp_fwd(Fwd& f, const FPBlk& b, Level& lv, PF cfeat, float4* dst, int Gd, int g_off) {
+  const int N = lv.n, M = lv.m, Gc = b.cc / 4, Gs = roundup(b.cp, 4) / 4;
+  const PF& skip = lv.feat;
   if (cfeat.G != Gc || cfeat.R != M) { set_error("FP: centre features mismatch"); return LION_ERR_ARG; }
   if (Gs && (skip.G != Gs || skip.R != N)) { set_error("FP: skip features mismatch (%d groups, expected %d)", skip.G, Gs); return LION_ERR_ARG; }
   size_t mk = f.c->mark();
-  const int* idx = pre_idx;
-  const float* wgt = pre_wgt;
-  if (idx) {                                      // 3-NN search already ran on the side stream
-    if (!f.c->dry) LION_CHECK_CUDA(cudaStreamWaitEvent(f.c->stream, f.c->ev[pre_ev], 0));
-  } else {
-    int* ii = f.c->alloc_n<int>((size_t)f.B * N * 3);
-    float* ww = f.c->alloc_n<float>((size_t)f.B * N * 3);
-    LION_LAUNCH(f.c, k_three_nn_c4, dim3(cdiv(N, 128), f.B), 128, 1024 * sizeof(float4), pts_c4, ctr_c4, ii, ww, N, M);
-    idx = ii; wgt = ww;
-  }
+  LION_TRY(wait_once(f.c, lv.nn_done));
   PF cat = alloc_pf(f, Gc + Gs, N);
-  LION_LAUNCH(f.c, k_interp_rows, dim3(cdiv(N, 128), Gc, f.B), 128, 0, cfeat.p, idx, wgt, cat.p, Gc, M, N, Gc + Gs, 0);
+  LION_LAUNCH(f.c, k_interp_rows, dim3(cdiv(N, 128), Gc, f.B), 128, 0, cfeat.p, lv.nn_idx, lv.nn_wgt, cat.p, Gc, M, N, Gc + Gs, 0);
   if (Gs) LION_LAUNCH(f.c, k_copy_groups, dim3(cdiv(N, 256), Gs, f.B), 256, 0, skip.p, cat.p, Gs, Gc + Gs, Gc, N);
   LION_TRY(check_launch(f.c, "fp interpolate"));
   LION_TRY(shared_mlp_fwd(f, b.mlp, cat, 1, dst, Gd, g_off));
   f.c->release(mk);
+  return 0;
+}
+
+// SA level i: its PVConvs on lv.pts, then its SA module onto lv.centers; feat is the level's input and becomes its
+// output.  Unless the caller has already planned the level's geometry (unet_forward, on the side stream), FPS and ball
+// query run here on the main stream, just before the SA module.
+static int sa_level_fwd(Fwd& f, const std::vector<Block>& blocks, Level& lv, PF& feat, int i) {
+  for (auto& blk : blocks) {
+    if (blk.kind == LION_KIND_PVCONV) {
+      PF o = alloc_pf(f, blk.pv.cout / 4, lv.n);
+      LION_TRY(pvconv_fwd(f, blk.pv, feat, lv.pts, o.p, o.G, 0));
+      feat = o;
+      stamp(f.c, f.c->stream, "sa.pvconv", i);
+      continue;
+    }
+    PF o = alloc_pf(f, blk.sa.mlp.cout() / 4, blk.sa.m);
+    const bool planned = lv.nidx != nullptr;
+    if (!planned) lv.centers = f.c->alloc_n<float4>((size_t)f.B * blk.sa.m);
+    const size_t mk = f.c->mark();
+    if (!planned) LION_TRY(sa_geometry(f, f.c->stream, blk.sa, lv, i));
+    LION_TRY(sa_fwd(f, blk.sa, feat, lv, o.p, o.G, 0));
+    f.c->release(mk);
+    feat = o;
+    stamp(f.c, f.c->stream, "sa.module", i);
+  }
   return 0;
 }
 
@@ -725,6 +777,7 @@ static int build_unet(Model* m, Cursor& cur) {
   int n_sa = 0;
   if (!(rd(u.num_classes) && rd(u.embed_dim) && rd(u.extra) && rd(u.input_dim) && rd(u.use_att) && rd(u.clip) &&
         rd(u.clip_dim) && rd(u.S) && rd(n_sa))) { set_error("unet descriptor too short"); return LION_ERR_ARG; }
+  if (n_sa < 1) { set_error("unet: at least one SA level"); return LION_ERR_ARG; }
   m->S = u.S;
   int E = u.embed_dim;
   if (u.input_dim != 3 || u.extra < 0 || u.extra > 1) { set_error("unet: points must be xyz + at most one extra feature channel"); return LION_ERR_ARG; }
@@ -746,6 +799,7 @@ static int build_unet(Model* m, Cursor& cur) {
   if (u.use_att) LION_TRY(make_attn(m, u.gatt, cur, ch_sa, 8));
   int n_fp = 0;
   if (!rd(n_fp)) { set_error("unet descriptor truncated (fp)"); return LION_ERR_ARG; }
+  if (n_fp > n_sa) { set_error("unet: %d FP stages for %d SA levels", n_fp, n_sa); return LION_ERR_ARG; }
   for (int i = 0; i < n_fp; ++i) {
     int nm;
     if (!rd(nm)) { set_error("unet descriptor truncated (fp)"); return LION_ERR_ARG; }
@@ -768,6 +822,20 @@ static int build_unet(Model* m, Cursor& cur) {
     }
     u.fp.push_back(std::move(blocks));
   }
+  // per point level: the voxel preps of the PVConvs on its points (SA level l's, then FP stage n_sa - 1 - l's) and the
+  // events of what the side stream computes for it
+  u.levels.resize(n_sa);
+  for (int l = 0; l < n_sa; ++l) {
+    UnetLevel& lv = u.levels[l];
+    auto add_r = [&](const std::vector<Block>& blocks) {
+      for (auto& b : blocks)
+        if (b.kind == LION_KIND_PVCONV && std::find(lv.vox_r.begin(), lv.vox_r.end(), b.pv.r) == lv.vox_r.end()) lv.vox_r.push_back(b.pv.r);
+    };
+    add_r(u.sa[l]);
+    if (n_sa - 1 - l < n_fp) add_r(u.fp[n_sa - 1 - l]);
+    for (cudaEvent_t* e : {&lv.sa_done, &lv.vox_done, &lv.nn_done}) LION_TRY(m->make_event(e));
+  }
+  for (cudaEvent_t* e : {&u.aux_start, &u.temb_done}) LION_TRY(m->make_event(e));
   // classifier: SharedMLP(ch_fp -> 128), Dropout, Conv1d(128 -> num_classes) (latent_points_ada.py:94-99)
   LION_TRY(make_shared_mlp(m, u.cls0, cur, in_ch, ident_map(in_ch), {128}));
   const float* cw = cur.next(); const float* cb = cur.next();
@@ -812,24 +880,15 @@ static int style_enc_forward(Fwd& f, const float* x, float* out, int N) {
   LION_TRY(style_affine_all(f, dummy_style));
   LION_TRY(stat_pool_begin(f, (size_t)f.m->style_total * B * sizeof(double) + 4096));
   PF feat; feat.p = c0; feat.G = 1; feat.R = N;
-  const float4* coords = c0;
-  int Ncur = N;
-  for (auto& lvl : e.sa) {
-    for (auto& blk : lvl) {
-      if (blk.kind == LION_KIND_PVCONV) {
-        PF o = alloc_pf(f, blk.pv.cout / 4, Ncur);
-        LION_TRY(pvconv_fwd(f, blk.pv, feat, coords, o.p, o.G, 0));
-        feat = o;
-      } else {
-        PF o = alloc_pf(f, blk.sa.mlp.cout() / 4, blk.sa.m);
-        float4* ctr = c->alloc_n<float4>((size_t)B * blk.sa.m);
-        LION_TRY(sa_fwd(f, blk.sa, feat, coords, ctr, o.p, o.G, 0));
-        feat = o; coords = ctr; Ncur = blk.sa.m;
-      }
-    }
+  const float4* pts = c0;
+  int n = N;
+  for (size_t i = 0; i < e.sa.size(); ++i) {
+    Level lv{pts, n};
+    LION_TRY(sa_level_fwd(f, e.sa[i], lv, feat, (int)i));
+    pts = lv.centers; n = lv.m;
   }
   float* pooled = c->alloc_n<float>((size_t)B * e.cfeat);
-  LION_LAUNCH(c, k_max_rows, dim3(feat.G, B), 256, 0, feat.p, pooled, feat.G, Ncur);
+  LION_LAUNCH(c, k_max_rows, dim3(feat.G, B), 256, 0, feat.p, pooled, feat.G, n);
   LION_LAUNCH(c, k_small_linear, B, 128, e.cfeat * sizeof(float), e.mlp_w, e.mlp_b, pooled, e.cfeat, out, 2 * e.zdim, e.cfeat, 2 * e.zdim, 0);
   return check_launch(c, "style encoder");
 }
@@ -852,20 +911,70 @@ static int unet_style_affine(Fwd& f, const float* style, const float* clip) {
   return style_affine_all(f, style);
 }
 
+// Everything of a U-Net forward that depends on coordinates (and t) only runs on the side stream, in this order: per SA
+// level i its FPS and ball query, the time embedding after level 0, the voxel preps of level i + 1's points; then the
+// FP stages' 3-NN searches from the deepest level up.  FPS alone is a chain of ~1360 latency-bound rounds on 32 SMs:
+// there it hides under the first PVConvs.  The main stream waits for each result where it first needs it.
+// Every buffer written on aux is allocated here, before the main stream's first mark(): no release() on the main
+// stream can hand it to another buffer while aux may still be writing it.
+static int unet_side_stream(Fwd& f, const float* t, float* temb, std::vector<Level>& L, cudaEvent_t& temb_done) {
+  UnetBlk& u = *f.m->unet;
+  Ctx* c = f.c;
+  const int B = f.B, E = u.embed_dim, n_sa = (int)L.size();
+  if (!c->dry) {
+    LION_CHECK_CUDA(cudaEventRecord(u.aux_start, c->stream));
+    LION_CHECK_CUDA(cudaStreamWaitEvent(c->aux, u.aux_start, 0));
+    static DevOnce carve_once;
+    if (carve_once.need()) {     // side-stream kernels share SMs with the convolutions: same (maximum) carve-out
+      LION_CHECK_CUDA(cudaFuncSetAttribute(k_ball_query_c4, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      LION_CHECK_CUDA(cudaFuncSetAttribute(k_three_nn_c4, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
+  }
+  for (int i = 0; i < n_sa; ++i) {
+    const SABlk& sb = u.sa[i].back().sa;
+    L[i].centers = c->alloc_n<float4>((size_t)B * sb.m);
+    LION_TRY(sa_geometry(f, c->aux, sb, L[i], i));
+    LION_TRY(record_on_aux(c, u.levels[i].sa_done, L[i].sa_done));
+    if (i == 0 && temb) {
+      // three tiny dependent launches (~45 us of latency) that nothing needs before level 1
+      float* sinu = c->alloc_n<float>((size_t)B * E);
+      float* h = c->alloc_n<float>((size_t)B * E);
+      LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, sinu, E / 2, 1.0f);
+      LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e0w, u.e0b, sinu, E, h, E, E, E, 1);
+      LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e2w, u.e2b, h, E, temb, E, E, E, 0);
+      stamp(c, c->aux, "temb");
+      LION_TRY(record_on_aux(c, u.temb_done, temb_done));
+    }
+    if (i + 1 == n_sa) continue;
+    // the centres are level i + 1's points; voxelising them depends on coordinates only -- one CTA per shape, 13-25 us
+    // each on the critical path otherwise
+    Level& next = L[i + 1];
+    next.pts = L[i].centers; next.n = sb.m;
+    const std::vector<int>& rs = u.levels[i + 1].vox_r;
+    for (int r : rs) { VoxPrep* vp; LION_TRY(get_vox(f, c->aux, next.pts, next.n, r, &vp)); }
+    if (!rs.empty()) {
+      stamp(c, c->aux, "voxprep", i + 1);
+      LION_TRY(record_on_aux(c, u.levels[i + 1].vox_done, next.vox_done));
+    }
+  }
+  for (int j = 0; j < (int)u.fp.size(); ++j) {
+    const int l = n_sa - 1 - j;                     // FP stage j interpolates back onto level l's points
+    LION_TRY(fp_geometry(f, c->aux, L[l], l));
+    LION_TRY(record_on_aux(c, u.levels[l].nn_done, L[l].nn_done));
+  }
+  return 0;
+}
+
 static int unet_forward(Fwd& f, const float* x, const float* t, const float* style, const float* clip, float* out, int N) {
   UnetBlk& u = *f.m->unet;
   int B = f.B, E = u.embed_dim;
   Ctx* c = f.c;
-  // time embedding: sinusoid -> Linear -> LeakyReLU(0.1) -> Linear  (latent_points_ada.py:53-57, :101-128)
+  // time embedding: sinusoid -> Linear -> LeakyReLU(0.1) -> Linear  (latent_points_ada.py:53-57, :101-128), computed
+  // on the side stream
   float* temb = nullptr;
-  float *temb_sinu = nullptr, *temb_h = nullptr;
-  bool temb_pending = false;
   if (E > 0) {
     if (!t) { set_error("unet: this network needs timesteps"); return LION_ERR_ARG; }
-    float* sinu = c->alloc_n<float>((size_t)B * E);
-    float* h = c->alloc_n<float>((size_t)B * E);
     temb = c->alloc_n<float>((size_t)B * E);
-    temb_sinu = sinu; temb_h = h;       // launched below, on the side stream: first used at SA level 1
   }
   // AdaGN style Linears (and the CLIP mixing in front of them) depend on the style only, which is constant over the
   // 1000 steps of a sampling run: style == nullptr means "use what lion_unet_cache_style computed"
@@ -878,10 +987,7 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
   LION_TRY(check_launch(c, "unet prologue"));
   LION_TRY(stat_pool_begin(f, (size_t)f.m->style_total * f.B * sizeof(double) + 4096));   // sum(2*C) doubles per shape
 
-  int n_sa = (int)u.sa.size();
-  std::vector<const float4*> coords_list(n_sa);
-  std::vector<PF> feats_list(n_sa);
-  std::vector<int> n_list(n_sa);
+  const int n_sa = (int)u.sa.size();
   // level-0 inputs: coords = xyz, features = all input channels (the latent x[B,N,4] itself is a PF with G=1; a
   // 3-channel cloud x[B,N,3] (PointTransPVC) is padded to (x, y, z, 0), which serves as coordinates AND features)
   float4* c0 = c->alloc_n<float4>((size_t)B * N);
@@ -893,94 +999,13 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
     LION_LAUNCH(c, k_make_coords, cdiv(B * N, 256), 256, 0, (const float4*)x, c0, B * N);
     feat.p = (float4*)x;
   }
-  // furthest-point sampling of all levels depends on coordinates only: a chain of 1360 latency-
-  // bound rounds on 32 SMs.  Fork it onto the side stream so it hides under the first PVConvs.
-  std::vector<float4*> fps_centers(n_sa, nullptr);
-  // Neighbour searches depend on coordinates only as well: the ball query of level i follows FPS i on the side stream,
-  // the four 3-NN searches of the FP half follow the last FPS.
-  const bool side_nn = n_sa <= 4;
-  std::vector<int*> sa_nidx(n_sa, nullptr), fp_idx(n_sa, nullptr);
-  std::vector<char> vox_pending(n_sa + 1, 0);
-  std::vector<float*> fp_wgt(n_sa, nullptr);
-  {
-    const float4* src = c0;
-    int ncur = N;
-    if (!c->dry) {
-      LION_CHECK_CUDA(cudaEventRecord(c->ev_fork, c->stream));
-      LION_CHECK_CUDA(cudaStreamWaitEvent(c->aux, c->ev_fork, 0));
-      static DevOnce carve_once;
-      if (carve_once.need()) {     // side-stream kernels share SMs with the convolutions: same (maximum) carve-out
-        LION_CHECK_CUDA(cudaFuncSetAttribute(k_ball_query_c4, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        LION_CHECK_CUDA(cudaFuncSetAttribute(k_three_nn_c4, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-      }
-    }
-    for (int i = 0; i < n_sa && i < 8; ++i) {
-      const SABlk& sb = u.sa[i].back().sa;
-      if (ncur > FPS_MAX_N || sb.m > ncur) { set_error("unet: FPS sizes unsupported"); return LION_ERR_ARG; }
-      fps_centers[i] = c->alloc_n<float4>((size_t)B * sb.m);
-      int* fidx = c->alloc_n<int>((size_t)B * sb.m);
-      LION_TRY(fps_c4(c, c->aux, B, src, fidx, fps_centers[i], ncur, sb.m));
-      stamp(c, c->aux, "aux:fps", i);
-      if (side_nn) {
-        sa_nidx[i] = c->alloc_n<int>((size_t)B * sb.m * sb.k);
-        LION_LAUNCH_ON(c, c->aux, k_ball_query_c4, dim3(cdiv(sb.m * 32, 256), B), 256, 0, fps_centers[i], src, sa_nidx[i], ncur, sb.m,
-                       sb.radius * sb.radius, sb.k);
-        stamp(c, c->aux, "aux:ballq", i);
-      }
-      if (!c->dry) LION_CHECK_CUDA(cudaEventRecord(c->ev[i], c->aux));
-      if (i == 0 && temb) {
-        // three tiny dependent launches (~45 us of latency) that nothing needs before level 1
-        LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, temb_sinu, E / 2, 1.0f);
-        LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e0w, u.e0b, temb_sinu, E, temb_h, E, E, E, 1);
-        LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e2w, u.e2b, temb_h, E, temb, E, E, E, 0);
-        stamp(c, c->aux, "aux:temb");
-        if (!c->dry) {
-          LION_CHECK_CUDA(cudaEventRecord(c->ev_temb, c->aux));
-          temb_pending = true;
-        }
-      }
-      // voxelisation prep of the PVConvs that work on these centres (the next SA level and, mirrored, an FP level):
-      // it depends on coordinates only -- one CTA per shape, 13-25 us each on the critical path otherwise
-      if (side_nn) {
-        int rs[2] = {0, 0};
-        if (i + 1 < n_sa) for (auto& blk : u.sa[i + 1]) if (blk.kind == LION_KIND_PVCONV) rs[0] = blk.pv.r;
-        const int fi = n_sa - 2 - i;                  // FP stage whose PVConvs run on level i + 1's points
-        if (fi >= 0 && fi < (int)u.fp.size()) for (auto& blk : u.fp[fi]) if (blk.kind == LION_KIND_PVCONV) rs[1] = blk.pv.r;
-        bool any = false;
-        for (int k = 0; k < 2; ++k) {
-          if (rs[k] <= 0 || (k == 1 && rs[1] == rs[0])) continue;
-          VoxPrep* vp = nullptr;
-          LION_TRY(get_vox(f, c->aux, fps_centers[i], sb.m, rs[k], &vp));
-          any = true;
-        }
-        if (any && !c->dry) {
-          stamp(c, c->aux, "aux:voxprep", i + 1);
-          LION_CHECK_CUDA(cudaEventRecord(c->ev_vox[i], c->aux));
-          vox_pending[i + 1] = true;
-        }
-      }
-      src = fps_centers[i];
-      ncur = sb.m;
-    }
-    if (side_nn && u.fp.size() == (size_t)n_sa) {
-      for (int lvl = n_sa - 1; lvl >= 0; --lvl) {
-        const float4* pts = lvl == 0 ? c0 : fps_centers[lvl - 1];
-        const int npts = lvl == 0 ? N : u.sa[lvl - 1].back().sa.m, nctr = u.sa[lvl].back().sa.m;
-        fp_idx[lvl] = c->alloc_n<int>((size_t)B * npts * 3);
-        fp_wgt[lvl] = c->alloc_n<float>((size_t)B * npts * 3);
-        LION_LAUNCH_ON(c, c->aux, k_three_nn_c4, dim3(cdiv(npts, 128), B), 128, 1024 * sizeof(float4), pts, fps_centers[lvl], fp_idx[lvl],
-                       fp_wgt[lvl], npts, nctr);
-        stamp(c, c->aux, "aux:3nn", lvl);
-        if (!c->dry) LION_CHECK_CUDA(cudaEventRecord(c->ev[4 + lvl], c->aux));
-      }
-    }
-  }
+  std::vector<Level> L(n_sa);
+  L[0].pts = c0; L[0].n = N;
+  cudaEvent_t temb_done = nullptr;
+  LION_TRY(unet_side_stream(f, t, temb, L, temb_done));
   stamp(c, c->stream, "start");
-  const float4* coords = c0;
-  int Ncur = N;
-  bool has_t = temb != nullptr;
   auto with_temb = [&](PF src, PF* dstp) -> int {   // cat(features, temb expanded) (:145)
-    if (temb_pending) { LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, c->ev_temb, 0)); temb_pending = false; }
+    LION_TRY(wait_once(c, temb_done));
     PF d = alloc_pf(f, src.G + E / 4, src.R);
     LION_LAUNCH(c, k_copy_groups, dim3(cdiv(src.R, 256), src.G, B), 256, 0, src.p, d.p, src.G, d.G, 0, src.R);
     LION_LAUNCH(c, k_fill_groups, dim3(cdiv(src.R, 256), E / 4, B), 256, 0, temb, E, d.p, d.G, src.G, src.R);
@@ -991,70 +1016,51 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
   constexpr int CONV_SMEM_BESIDE_AUX = 196 * 1024;
   for (int i = 0; i < n_sa; ++i) {
     c->conv_smem_cap = i == 0 ? CONV_SMEM_BESIDE_AUX : 0;      // the side stream is busy during level 0
-    feats_list[i] = feat; coords_list[i] = coords; n_list[i] = Ncur;
-    if (vox_pending[i]) { LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, c->ev_vox[i - 1], 0)); vox_pending[i] = 0; }
-    if (i > 0 && has_t) LION_TRY(with_temb(feat, &feat));
-    for (auto& blk : u.sa[i]) {
-      if (blk.kind == LION_KIND_PVCONV) {
-        PF o = alloc_pf(f, blk.pv.cout / 4, Ncur);
-        LION_TRY(pvconv_fwd(f, blk.pv, feat, coords, o.p, o.G, 0));
-        feat = o;
-        stamp(c, c->stream, "sa.pvconv", i);
-      } else {
-        PF o = alloc_pf(f, blk.sa.mlp.cout() / 4, blk.sa.m);
-        float4* ctr = fps_centers[i];
-        LION_TRY(sa_fwd(f, blk.sa, feat, coords, ctr, o.p, o.G, 0, i, sa_nidx[i]));
-        feat = o; coords = ctr; Ncur = blk.sa.m;
-        stamp(c, c->stream, "sa.module", i);
-      }
-    }
+    L[i].feat = feat;
+    LION_TRY(wait_once(c, L[i].vox_done));
+    if (i > 0 && temb) LION_TRY(with_temb(feat, &feat));
+    LION_TRY(sa_level_fwd(f, u.sa[i], L[i], feat, i));
   }
   c->conv_smem_cap = 0;
   // skip features of level 0 are the extra channels only (inputs[:, 3:], :153): packed as
   // one group [f, 0, 0, 0]
-  if (u.extra == 1) {
-    PF s0 = alloc_pf(f, 1, N);
-    LION_LAUNCH(c, k_extract_extra, cdiv(B * N, 256), 256, 0, (const float4*)x, s0.p, B * N);
-    feats_list[0] = s0;
-  } else {
-    feats_list[0] = PF();          // no skip features at level 0
-  }
+  L[0].feat = u.extra == 1 ? alloc_pf(f, 1, N) : PF();
+  if (u.extra == 1) LION_LAUNCH(c, k_extract_extra, cdiv(B * N, 256), 256, 0, (const float4*)x, L[0].feat.p, B * N);
   if (u.use_att) {
-    PF o = alloc_pf(f, feat.G, Ncur);
+    PF o = alloc_pf(f, feat.G, feat.R);
     LION_TRY(attn_fwd(f, u.gatt, feat, o.p, o.G, 0));
     feat = o;
     stamp(c, c->stream, "global_att");
   }
-  for (size_t i = 0; i < u.fp.size(); ++i) {
-    int lvl = n_sa - 1 - (int)i;
-    for (auto& blk : u.fp[i]) {
+  for (size_t j = 0; j < u.fp.size(); ++j) {
+    Level& lv = L[n_sa - 1 - j];
+    for (auto& blk : u.fp[j]) {
       if (blk.kind == LION_KIND_FP) {
         PF cf = feat;
-        if (has_t) LION_TRY(with_temb(feat, &cf));          // torch.cat([features, temb]) (:160)
-        PF o = alloc_pf(f, blk.fp.mlp.cout() / 4, n_list[lvl]);
-        LION_TRY(fp_fwd(f, blk.fp, coords_list[lvl], n_list[lvl], coords, Ncur, cf, feats_list[lvl], o.p, o.G, 0,
-                        fp_idx[lvl], fp_wgt[lvl], 4 + lvl));
-        feat = o; coords = coords_list[lvl]; Ncur = n_list[lvl];
-        stamp(c, c->stream, "fp.module", (int)i);
-      } else {
-        PF o = alloc_pf(f, blk.pv.cout / 4, Ncur);
-        LION_TRY(pvconv_fwd(f, blk.pv, feat, coords, o.p, o.G, 0));
+        if (temb) LION_TRY(with_temb(feat, &cf));          // torch.cat([features, temb]) (:160)
+        PF o = alloc_pf(f, blk.fp.mlp.cout() / 4, lv.n);
+        LION_TRY(fp_fwd(f, blk.fp, lv, cf, o.p, o.G, 0));
         feat = o;
-        stamp(c, c->stream, "fp.pvconv", (int)i);
+        stamp(c, c->stream, "fp.module", (int)j);
+      } else {
+        PF o = alloc_pf(f, blk.pv.cout / 4, lv.n);
+        LION_TRY(pvconv_fwd(f, blk.pv, feat, lv.pts, o.p, o.G, 0));
+        feat = o;
+        stamp(c, c->stream, "fp.pvconv", (int)j);
       }
     }
   }
-  PF h = alloc_pf(f, 32, Ncur);
+  PF h = alloc_pf(f, 32, feat.R);
   LION_TRY(shared_mlp_fwd(f, u.cls0, feat, 1, h.p, 32, 0));
   if (u.num_classes == 4) {
-    LION_TRY(run_conv(f, u.cls2, h.p, h.G, (float4*)out, 1, nullptr, nullptr, geom_rows(Ncur)));
+    LION_TRY(run_conv(f, u.cls2, h.p, h.G, (float4*)out, 1, nullptr, nullptr, geom_rows(feat.R)));
   } else {
-    PF o4 = alloc_pf(f, (u.num_classes + 3) / 4, Ncur);
-    LION_TRY(run_conv(f, u.cls2, h.p, h.G, o4.p, o4.G, nullptr, nullptr, geom_rows(Ncur)));
-    LION_LAUNCH(c, k_pf_to_pm, dim3(cdiv(Ncur, 256), o4.G, B), 256, 0, o4.p, out, o4.G, u.num_classes, Ncur);
+    PF o4 = alloc_pf(f, (u.num_classes + 3) / 4, feat.R);
+    LION_TRY(run_conv(f, u.cls2, h.p, h.G, o4.p, o4.G, nullptr, nullptr, geom_rows(feat.R)));
+    LION_LAUNCH(c, k_pf_to_pm, dim3(cdiv(feat.R, 256), o4.G, B), 256, 0, o4.p, out, o4.G, u.num_classes, feat.R);
   }
-  if (temb_pending) LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, c->ev_temb, 0));   // never consumed: still join the side stream
-  for (int i = 1; i <= n_sa; ++i) if (vox_pending[i]) LION_CHECK_CUDA(cudaStreamWaitEvent(c->stream, c->ev_vox[i - 1], 0));
+  // never consumed by a one-level network: still join the side stream (every other result was waited for above)
+  LION_TRY(wait_once(c, temb_done));
   stamp(c, c->stream, "end");
   return check_launch(c, "unet epilogue");
 }
@@ -1107,10 +1113,6 @@ extern "C" int lion_ctx_create(int device, LionCtx** out) {
   LION_CHECK_CUDA(cudaStreamCreateWithFlags(&h->c.aux, cudaStreamNonBlocking));
   { const char* e = getenv("LION_TIMELINE");
     if (e && atoi(e) != 0) LION_CHECK_CUDA(cudaMalloc(&h->c.d_stamps, LION_MAX_STAMPS * sizeof(unsigned long long))); }
-  LION_CHECK_CUDA(cudaEventCreateWithFlags(&h->c.ev_fork, cudaEventDisableTiming));
-  LION_CHECK_CUDA(cudaEventCreateWithFlags(&h->c.ev_temb, cudaEventDisableTiming));
-  for (int i = 0; i < 4; ++i) LION_CHECK_CUDA(cudaEventCreateWithFlags(&h->c.ev_vox[i], cudaEventDisableTiming));
-  for (int i = 0; i < 8; ++i) LION_CHECK_CUDA(cudaEventCreateWithFlags(&h->c.ev[i], cudaEventDisableTiming));
   if (prop.major != 9 || prop.minor != 0) {
     set_error("lion_b200 is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     delete h;
@@ -1125,10 +1127,6 @@ extern "C" int lion_ctx_destroy(LionCtx* h) {
   if (h->c.zgrid) cudaFree(h->c.zgrid);
   if (h->c.aux) cudaStreamDestroy(h->c.aux);
   if (h->c.d_stamps) cudaFree(h->c.d_stamps);
-  if (h->c.ev_fork) cudaEventDestroy(h->c.ev_fork);
-  if (h->c.ev_temb) cudaEventDestroy(h->c.ev_temb);
-  for (int i = 0; i < 4; ++i) if (h->c.ev_vox[i]) cudaEventDestroy(h->c.ev_vox[i]);
-  for (int i = 0; i < 8; ++i) if (h->c.ev[i]) cudaEventDestroy(h->c.ev[i]);
   delete h;
   return 0;
 }
@@ -1315,12 +1313,13 @@ extern "C" int lion_sa_module_fwd(LionModel* h, const float* features, const flo
     const SABlk& s = m->block->sa;
     LION_TRY(style_affine_all(f, style ? style : f.c->alloc_n<float>((size_t)B * 4)));
     PF x = to_pf(f, features, s.cfeat, N);
-    float4* c4 = to_c4(f, coords, N);
-    float4* ctr = f.c->alloc_n<float4>((size_t)B * s.m);
+    Level lv{to_c4(f, coords, N), N};
+    lv.centers = f.c->alloc_n<float4>((size_t)B * s.m);
     PF o = alloc_pf(f, s.mlp.cout() / 4, s.m);
-    LION_TRY(sa_fwd(f, s, x, c4, ctr, o.p, o.G, 0));
+    LION_TRY(sa_geometry(f, f.c->stream, s, lv, 0));
+    LION_TRY(sa_fwd(f, s, x, lv, o.p, o.G, 0));
     from_pf(f, o, out_features, s.mlp.cout());
-    LION_LAUNCH(f.c, k_c4_to_cm, dim3(cdiv(s.m, 256), B), 256, 0, ctr, out_coords, s.m);
+    LION_LAUNCH(f.c, k_c4_to_cm, dim3(cdiv(s.m, 256), B), 256, 0, lv.centers, out_coords, s.m);
     return check_launch(f.c, "lion_sa_module_fwd");
   });
 }
@@ -1335,13 +1334,13 @@ extern "C" int lion_fp_module_fwd(LionModel* h, const float* points_coords, cons
   return two_pass(m, stream, B, [&](Fwd& f) {
     const FPBlk& b = m->block->fp;
     LION_TRY(style_affine_all(f, style));
-    float4* pc = to_c4(f, points_coords, N);
-    float4* cc = to_c4(f, centers_coords, M);
+    Level lv{to_c4(f, points_coords, N), N};
+    lv.centers = to_c4(f, centers_coords, M); lv.m = M;
     PF cf = to_pf(f, centers_features, b.cc, M);
-    PF sk;
-    if (b.cp) sk = to_pf(f, points_features, b.cp, N);
+    if (b.cp) lv.feat = to_pf(f, points_features, b.cp, N);
     PF o = alloc_pf(f, b.mlp.cout() / 4, N);
-    LION_TRY(fp_fwd(f, b, pc, N, cc, M, cf, sk, o.p, o.G, 0));
+    LION_TRY(fp_geometry(f, f.c->stream, lv, 0));
+    LION_TRY(fp_fwd(f, b, lv, cf, o.p, o.G, 0));
     from_pf(f, o, out, b.mlp.cout());
     return check_launch(f.c, "lion_fp_module_fwd");
   });
