@@ -7,23 +7,33 @@
 //
 // Formulation (im2col-free implicit GEMM on the zero-haloed packed layouts, see
 // packed_kernels.cuh):  out[p][co] = sum_tap sum_ci in[p + off(tap)][ci] * W[tap][ci][co].
-//   * M = 128 consecutive rows p of one shape (voxel positions incl. y/z halo rows, masked at
-//     the store), split into two 64-row halves, one per consumer warpgroup; N = output channels
-//     (<= 128 per CTA), K = 8 channels per wgmma.
+//   * M = 64 rows per wgmma, one block per consumer warpgroup; N = output channels (<= 128 per CTA), K = 8 channels
+//     per wgmma.  Row tiles (1x1, and 3x3x3 with N <= 64): a block is 64 consecutive rows, two make a 128-row tile, and
+//     3x3x3 halo rows inside it are computed and stored as zeros.  Interior blocks (3x3x3 with N = 128): a block is
+//     8 y-lines x 8 z of one x-plane -- halo rows are neither computed nor written.  Blocks are ordered z fastest, then
+//     y, then x, and a group of 2 consecutive blocks of one shape is one work item.
 //   * A operand: the activation tensor is [C/4][rows][4] in HBM, i.e. for 4 channels all rows
 //     are contiguous at a 16-byte pitch.  That *is* the canonical no-swizzle K-major wgmma
-//     layout (core matrix = 8 rows x 16 B = 128 contiguous bytes, SBO = 128 B between 8-row
-//     groups, LBO = distance between channel groups), so one contiguous cp.async.bulk per
-//     channel group stages 128 + 2*halo rows, and every one of the 9 (dy,dz) taps of an x-plane
-//     is the SAME shared-memory bytes viewed through a descriptor whose start address is
-//     shifted by (dy*(r+2)+dz) rows.  L2->SM traffic per MAC drops 9x versus reloading per tap.
+//     layout (core matrix = 8 rows x 16 B = 128 contiguous bytes, SBO between 8-row groups,
+//     LBO = distance between channel groups): SBO = 128 B covers 64 consecutive rows, SBO = (r+2) * 16 B covers
+//     8 consecutive y-lines of 8 z each.  One contiguous cp.async.bulk per channel group stages a 3x3x3 group's
+//     window for one x-plane tap (from row (y0-1, z0-1) of its first block to (y0+8, z0+8) of its last: 10 y-lines x
+//     18 z for 2 blocks at r = 16), and every one of the 9 (dy,dz) taps of every block is the SAME shared-memory
+//     bytes viewed through a descriptor whose start address is shifted by (dy*(r+2)+dz) rows.  L2->SM traffic per
+//     MAC drops 9x versus reloading per tap.
 //   * B operand: weights pre-packed [n-tile][chunk][x-plane][tap][C/4][co][4] so one bulk copy
 //     brings the 9 taps of a (channel chunk, x-plane); a CTA reuses it for up to tiles_per_item
-//     row tiles, whose accumulators all stay in registers (<= 128 per thread).
+//     blocks per warpgroup, whose accumulators all stay in registers (<= 128 per thread).
+//   * Output contract: rows of [p_begin, p_end) are written (halo rows as zeros), except on interior blocks, which
+//     leave the halo rows as they were: every consumer of a 3x3x3 output reads interior rows only.  Each output's
+//     accumulation order is the row tiles' (same channel chunks, x-planes, taps, k-steps), and the GroupNorm sums of
+//     interior blocks come from k_conv_stats in the row tiles' grouping: results are identical either way.
 //   * persistent CTAs (one per SM, 288 threads): warps 0-7 = two consumer warpgroups (wgmma into
-//     registers, then the epilogue: +bias -> halo mask -> coalesced float4 stores, GroupNorm sum /
+//     registers, then the epilogue: +bias -> row mask -> coalesced float4 stores, GroupNorm sum /
 //     sum-of-squares per warp in shared memory, one fp64 atomic per channel per shape and item),
 //     warp 8 = bulk-copy producer.
+#include <algorithm>
+
 #include "common.cuh"
 #include "model.cuh"
 #include "wgmma.cuh"
@@ -36,7 +46,7 @@ using namespace sm90;
 constexpr int CONSUMER_WARPS = 8;                    // two warpgroups: rows 0-63 / 64-127 of every tile
 constexpr int THREADS = 32 * CONSUMER_WARPS + 32;    // + warp 8, the producer
 constexpr int MAX_A_STAGES = 16;   // the A ring is as deep as shared memory allows (Params::a_stages)
-constexpr int B_STAGES = 2;
+constexpr int MAX_B_STAGES = 4;   // the weight ring: 2 slabs, deeper for 3x3x3 where shared memory allows (Params::b_stages)
 constexpr int OCC_SMEM = 1024;       // bytes of per-item occupancy flags kept in shared memory (r <= 38)
 // row tiles per work item: their accumulators (NT / 2 registers per thread each, 64 in all) share one weight slab.  The
 // block's 288 threads get at most 168 registers each; more accumulators spill.
@@ -54,18 +64,21 @@ struct Params {
   const float4* in; const float* w; const float* bias; float4* out; double* ssum; double* ssq;
   int Gin, Gout_store, cout_pad;
   int rows;              // rows per (b, group)
-  int p_begin, p_end;
-  int rp;                // r+2 (halo mask) or 0
+  int p_begin, p_end;    // 1x1: the rows computed
+  int ntile;             // tiles per shape: 1x1 128-row tiles, 3x3x3 block groups (see k_conv_tc)
   int ntg, tpg;          // tap groups (x planes) and taps per group: (3,9) or (1,1)
   int tg_off[3];         // row offset of each tap group (dx * rp^2)
   int tap_off[9];        // row offset of each tap inside a group (dy*rp + dz)
-  int halo;              // rp+1 or 0
+  // 3x3x3 block geometry: r, rp = r+2, z / y blocks per x plane (ceil(r/8)), blocks per shape, blocks per group
+  int r, rp, nzb, npl, nblk, ib;
+  int halo;              // 3x3x3 row tiles: rp+1 rows before and after the tile in the operand slab, else 0
   int KG, nchunk;        // channel groups per chunk, chunks
   int NT;                // output channels per CTA (wgmma N)
-  int G;                 // row tiles per work item
+  int G;                 // tiles per work item (1 for 3x3x3: a block group is one item)
   int B;                 // shapes
   int a_stage_bytes, b_stage_bytes, stage_rows;
   int a_stages;          // depth of the A ring
+  int b_stages;          // depth of the weight ring
   const unsigned char* occ;   // 64-row occupancy flags of the input (sparse first conv of a PVConv) or null
   int occ_stride;
   // pooled 1x1 (last layer of a set-abstraction MLP): instead of the [rows][C] result, write per 32 consecutive rows (the
@@ -78,10 +91,18 @@ struct Params {
   int sched;             // work distribution: 0 contiguous range per CTA, 1 interleaved items (see k_conv_tc)
 };
 
-// all wgmmas of one (row tile, channel chunk, tap group) for this warpgroup's 64 rows: TPG taps x KG/2 k-steps
+// 3x3x3: first row of block k of a shape (8 y-lines x 8 z of one x plane; blocks ordered z fastest, then y, then x)
+__host__ __device__ __forceinline__ int block_row(int k, int rp, int nzb, int npl) {
+  const int x = k / npl, rem = k - x * npl, yb = rem / nzb, zb = rem - yb * nzb;
+  return ((x + 1) * rp + 1 + 8 * yb) * rp + 1 + 8 * zb;
+}
+
+// all wgmmas of one (64-row block, channel chunk, tap group) for this warpgroup: TPG taps x KG/2 k-steps.  a_sbo is the
+// distance between the block's 8-row groups: 128 B for 64 consecutive rows, (r+2) * 16 B for 8 y-lines x 8 z.
 template <int KG, int TPG, int NT>
-__device__ __forceinline__ void issue_stage(float* d, uint32_t a_addr, uint32_t b_addr, uint32_t a_pitch, const int* tap_off) {
-  const uint64_t a0 = make_desc(a_addr, a_pitch, 128), b0 = make_desc(b_addr, NT * 16, 128);
+__device__ __forceinline__ void issue_stage(float* d, uint32_t a_addr, uint32_t b_addr, uint32_t a_pitch, uint32_t a_sbo,
+                                            const int* tap_off) {
+  const uint64_t a0 = make_desc(a_addr, a_pitch, a_sbo), b0 = make_desc(b_addr, NT * 16, 128);
 #pragma unroll
   for (int t = 0; t < TPG; ++t) {
     const uint64_t at = a0 + (uint64_t)(int64_t)(TPG == 1 ? 0 : tap_off[t]);      // descriptor address unit = 16 B = 1 row
@@ -92,7 +113,57 @@ __device__ __forceinline__ void issue_stage(float* d, uint32_t a_addr, uint32_t 
 }
 
 
-template <int KG, int TPG, int NT>
+struct Items {
+  long long u, u_end; int ntile_total, B, G;
+  int mode, m, q, n_p, n_q, c_i, i, big, k;   // sched 1: [u, u_end) is the rest of the current item (cut at n-tile boundaries)
+  // next item: n-tile nt, first tile v0 in the n-tile's flat (shape, row tile) space, ntile tiles.  An item may run
+  // across a shape boundary -- its tiles share the weight slabs whatever shape they belong to -- but not across n-tiles.
+  __device__ __forceinline__ bool next(int& nt, long long& v0, int& ntile) {
+    const long long per_nt = (long long)B * ntile_total;
+    if (mode) {
+      while (u >= u_end) {
+        if (k >= m) return false;
+        const int a0 = q * k / m, a1 = q * (k + 1) / m, b0 = (q + 1) * k / m, b1 = (q + 1) * (k + 1) / m;
+        u = (long long)n_q * a0 + (long long)n_p * b0 + (long long)(i - c_i) * (a1 - a0) + (long long)c_i * (b1 - b0);
+        u_end = u + (big ? b1 - b0 : a1 - a0);
+        ++k;
+      }
+      nt = (int)(u / per_nt);
+      v0 = u - (long long)nt * per_nt;
+      const long long lim = (long long)(nt + 1) * per_nt;
+      const long long e = u_end < lim ? u_end : lim;
+      ntile = (int)(e - u);          // <= ceil((q + 1) / m) <= G
+      u = e;
+      return true;
+    }
+    if (u >= u_end) return false;
+    nt = (int)(u / per_nt);
+    v0 = u - (long long)nt * per_nt;
+    long long run = per_nt - v0;
+    if (u_end - u < run) run = u_end - u;
+    const long long k2 = (run + G - 1) / G;
+    ntile = (int)((run + k2 - 1) / k2);
+    u += ntile;
+    return true;
+  }
+};
+// the items of CTA blockIdx.x out of gridDim.x over U = n-tiles x shapes x tiles (see k_conv_tc: work distribution)
+__device__ __forceinline__ Items make_items(long long U, int ntile_total, int B, int G, int sched) {
+  const long long u_begin = U * blockIdx.x / gridDim.x, u_end = U * (blockIdx.x + 1) / gridDim.x;
+  Items it{u_begin, u_end, ntile_total, B, G, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  if (sched) {
+    const int grid = (int)gridDim.x, q = (int)(U / grid), n_p = (int)(U - (long long)q * grid);
+    const int tmax = q + (n_p ? 1 : 0);
+    it.mode = 1; it.u = 0; it.u_end = 0;
+    it.m = (tmax + G - 1) / G; it.q = q; it.n_p = n_p; it.n_q = grid - n_p;
+    it.i = (int)blockIdx.x; it.c_i = (int)(u_begin - (long long)q * blockIdx.x);
+    it.big = (int)(u_end - u_begin) > q; it.k = 0;
+  }
+  return it;
+}
+
+// BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), otherwise 128-row tiles
+template <int KG, int TPG, int NT, bool BLK>
 __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   constexpr int GT = tiles_per_item(NT);
   constexpr int NACC = NT / 2;                  // accumulator registers per thread and tile
@@ -100,6 +171,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   uint8_t* sA = smem;
   const int A_STAGES = P.a_stages;
   uint8_t* sB = sA + (size_t)A_STAGES * P.a_stage_bytes;
+  const int B_STAGES = P.b_stages;
   float* s_bias = (float*)(sB + (size_t)B_STAGES * P.b_stage_bytes);
   float* s_stat = s_bias + 128;                 // [8 consumer warps][2][NT]: running GroupNorm partials of the current shape
   float* s_pool = s_stat + CONSUMER_WARPS * 2 * NT;    // [8 consumer warps][2][NT]: pooled-epilogue exchange (TPG == 1)
@@ -109,7 +181,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   const uint32_t bar_full_a = smem_u32(bars), bar_empty_a = smem_u32(bars + MAX_A_STAGES);
-  const uint32_t bar_full_b = smem_u32(bars + 2 * MAX_A_STAGES), bar_empty_b = smem_u32(bars + 2 * MAX_A_STAGES + B_STAGES);
+  const uint32_t bar_full_b = smem_u32(bars + 2 * MAX_A_STAGES), bar_empty_b = smem_u32(bars + 2 * MAX_A_STAGES + MAX_B_STAGES);
 
   // zero the A stages once: channel-group slots that a partial chunk does not load must hold
   // finite values (their weights are zero)
@@ -125,8 +197,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy zero fill -> async proxy readers
   __syncthreads();
 
-  // Work distribution.  The (n-tile, shape, row-tile) space is flattened (row tile fastest) and cut into work items = up to G
-  // consecutive row tiles sharing the weight slabs (they may belong to two shapes, never to two n-tiles).  Every CTA gets
+  // Work distribution.  The (n-tile, shape, tile) space is flattened (tile fastest) and cut into work items = up to G
+  // consecutive tiles sharing the weight slabs (they may belong to two shapes, never to two n-tiles).  A 1x1 tile is 128
+  // consecutive rows; on interior blocks a tile is one group of ib blocks, and G = 1 (the group already shares the weight slabs and has
+  // one operand window, so it never spans two shapes).  3x3x3 tiles are ordered x-major like the rows.  Every CTA gets
   // the same number of tiles (+-1): fixed G-tile items dealt round-robin would leave some CTAs half again as many tiles as
   // others, and the kernel runs at the pace of the busiest.
   //   sched 0: one contiguous range per CTA, cut into evenly sized items (9 tiles -> 3+3+3, not 4+4+1).  Balanced, but at
@@ -138,53 +212,10 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   //            (a few shapes), so a tile's x-plane neighbours are in flight in a neighbouring CTA and hit the L2.
   //            With T_i in {q, q+1} every offset has a closed form: A_k = floor(q k / m), B_k = floor((q+1) k / m),
   //            c_i = CTAs before i that own q+1 tiles;  start(i, k) = n_q A_k + n_p B_k + (i - c_i)(A_k+1 - A_k) + c_i (B_k+1 - B_k).
-  const int ntile_total = (P.p_end - P.p_begin + 127) / 128;
+  const int ntile_total = P.ntile;
   const int n_nt = P.cout_pad / P.NT;
   const long long U = (long long)n_nt * P.B * ntile_total;
-  const long long u_begin = U * blockIdx.x / gridDim.x, u_end = U * (blockIdx.x + 1) / gridDim.x;
-  struct Items {
-    long long u, u_end; int ntile_total, B, G;
-    int mode, m, q, n_p, n_q, c_i, i, big, k;   // sched 1: [u, u_end) is the rest of the current item (cut at n-tile boundaries)
-    // next item: n-tile nt, first tile v0 in the n-tile's flat (shape, row tile) space, ntile tiles.  An item may run
-    // across a shape boundary -- its tiles share the weight slabs whatever shape they belong to -- but not across n-tiles.
-    __device__ __forceinline__ bool next(int& nt, long long& v0, int& ntile) {
-      const long long per_nt = (long long)B * ntile_total;
-      if (mode) {
-        while (u >= u_end) {
-          if (k >= m) return false;
-          const int a0 = q * k / m, a1 = q * (k + 1) / m, b0 = (q + 1) * k / m, b1 = (q + 1) * (k + 1) / m;
-          u = (long long)n_q * a0 + (long long)n_p * b0 + (long long)(i - c_i) * (a1 - a0) + (long long)c_i * (b1 - b0);
-          u_end = u + (big ? b1 - b0 : a1 - a0);
-          ++k;
-        }
-        nt = (int)(u / per_nt);
-        v0 = u - (long long)nt * per_nt;
-        const long long lim = (long long)(nt + 1) * per_nt;
-        const long long e = u_end < lim ? u_end : lim;
-        ntile = (int)(e - u);          // <= ceil((q + 1) / m) <= G
-        u = e;
-        return true;
-      }
-      if (u >= u_end) return false;
-      nt = (int)(u / per_nt);
-      v0 = u - (long long)nt * per_nt;
-      long long run = per_nt - v0;
-      if (u_end - u < run) run = u_end - u;
-      const long long k2 = (run + G - 1) / G;
-      ntile = (int)((run + k2 - 1) / k2);
-      u += ntile;
-      return true;
-    }
-  };
-  Items items0{u_begin, u_end, ntile_total, P.B, P.G, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  if (P.sched) {
-    const int grid = (int)gridDim.x, q = (int)(U / grid), n_p = (int)(U - (long long)q * grid);
-    const int tmax = q + (n_p ? 1 : 0);
-    items0.mode = 1; items0.u = 0; items0.u_end = 0;
-    items0.m = (tmax + P.G - 1) / P.G; items0.q = q; items0.n_p = n_p; items0.n_q = grid - n_p;
-    items0.i = (int)blockIdx.x; items0.c_i = (int)(u_begin - (long long)q * blockIdx.x);
-    items0.big = (int)(u_end - u_begin) > q; items0.k = 0;
-  }
+  const Items items0 = make_items(U, ntile_total, P.B, P.G, P.sched);
 
   if (warp == CONSUMER_WARPS) {
     // ===================== producer (whole warp; lane kg issues the copy of channel group kg) ====
@@ -216,7 +247,17 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
           if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
           for (int j = 0; j < ntile; ++j) {
             const int bj = __shfl_sync(0xffffffffu, my_b, j), tj = __shfl_sync(0xffffffffu, my_t, j);
-            const long long row0 = (long long)P.p_begin + (long long)tj * 128 - P.halo + P.tg_off[tg];
+            // row tiles: the tile's 128 rows (3x3x3: plus rp+1 halo rows on each side, shifted to x-plane tg).  Interior
+            // blocks: the window of block group tj under tap group tg, from one row before
+            // its first block's (-1, -1) neighbour; the last group's window is cut at the end of the shape's rows
+            long long row0;
+            uint32_t cnt = (uint32_t)P.stage_rows;
+            if (!BLK) {
+              row0 = (long long)P.p_begin + (long long)tj * 128 - P.halo + P.tg_off[tg];
+            } else {
+              row0 = (long long)block_row(tj * P.ib, P.rp, P.nzb, P.npl) - P.rp - 1 + P.tg_off[tg];
+              if (row0 + cnt > (long long)P.rows) cnt = (uint32_t)(P.rows - row0);
+            }
             const float4* in_lane = P.in + ((size_t)bj * P.Gin + grp_lane) * P.rows;
             mbar_wait(bar_empty_a + 8 * sa, pa ^ 1);
             bool empty = false;
@@ -233,7 +274,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
                 }
                 occ_b = s_occ;
               }
-              long long lo = row0 < 0 ? 0 : row0, hi = row0 + P.stage_rows - 1;
+              long long lo = row0 < 0 ? 0 : row0, hi = row0 + cnt - 1;
               if (hi > P.rows - 1) hi = P.rows - 1;
               unsigned any = 0;
               for (int k = (int)(lo >> 6); k <= (int)(hi >> 6); ++k) any |= occ_b[k];
@@ -243,24 +284,26 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
             if (lane == 0) {
               s_skip[sa] = empty ? 1u : 0u;
               if (empty) asm volatile("mbarrier.arrive.release.cta.shared::cta.b64 _, [%0];" ::"r"(full) : "memory");
-              else mbar_expect_tx(full, bytes * kg_real);
+              else mbar_expect_tx(full, cnt * 16u * kg_real);
             }
             __syncwarp();
             if (!empty && lane < kg_real)
-              bulk_g2s(sA_addr + sa * (uint32_t)P.a_stage_bytes + lane * bytes, in_lane + row0, bytes, full);
+              bulk_g2s(sA_addr + sa * (uint32_t)P.a_stage_bytes + lane * bytes, in_lane + row0, cnt * 16u, full);
             if (++sa == (uint32_t)A_STAGES) { sa = 0; pa ^= 1; }
           }
         }
       }
     }
   } else {
-    // ===================== consumers: warpgroup wg computes rows 64 wg .. 64 wg + 63 of every tile ===========
+    // ===================== consumers ===========
+    // row tiles: warpgroup wg computes rows 64 wg .. 64 wg + 63 of every tile.  Interior blocks: blocks wg, wg + 2, ...
     const int cw = warp, wg = cw >> 2, wq = cw & 3;
     const int et = tid;                                  // 0..255
     const uint32_t a_pitch = (uint32_t)P.stage_rows * 16u;
-    const uint32_t a_ring = smem_u32(sA) + (uint32_t)(P.halo + 64 * wg) * 16u;
+    const uint32_t a_sbo = BLK ? (uint32_t)P.rp * 16u : 128u;
+    const uint32_t a_ring = smem_u32(sA) + (BLK ? 0u : (uint32_t)(P.halo + 64 * wg) * 16u);
     const uint32_t b_ring = smem_u32(sB);
-    const int r_lo = 64 * wg + 16 * wq + (lane >> 2);   // this thread's rows of a tile: r_lo and r_lo + 8,
+    const int r_lo = 64 * wg + 16 * wq + (lane >> 2);   // 1x1: this thread's rows of a tile: r_lo and r_lo + 8,
     const int c_lo = 2 * (lane & 3);                     // its columns: 8 i + c_lo and 8 i + c_lo + 1
     const bool odd = (lane & 1) != 0;
     float acc[GT][NACC];
@@ -276,6 +319,23 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
       for (int j = 0; j < GT; ++j)
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[j][i] = 0.0f;
+      // 3x3x3: this warpgroup's nbw blocks of the group (first block g_f) and their offsets in the window.  All GT
+      // blocks are issued (a wgmma under a branch would serialise them all): a block past the shape's last one reads the
+      // group's first block, and its accumulators are not stored.
+      int g_f = 0, nbw = 0;
+      uint32_t boff[GT];
+      if (BLK) {
+        const int g_b = (int)(v0 / ntile_total);
+        g_f = (int)(v0 - (long long)g_b * ntile_total) * P.ib;
+        const int nb = min(P.ib, P.nblk - g_f);
+        nbw = (nb - wg + 1) / 2;
+        const int s_f = block_row(g_f, P.rp, P.nzb, P.npl);
+#pragma unroll
+        for (int j = 0; j < GT; ++j) {
+          const int k = 2 * j + wg < nb ? g_f + 2 * j + wg : g_f;
+          boff[j] = (uint32_t)(block_row(k, P.rp, P.nzb, P.npl) - s_f + P.rp + 1) * 16u;
+        }
+      }
       // A stage (and weight slab) handed back one commit group late (wait_group 1): the tensor cores work on the
       // next stage while this warp checks that the previous one has been read
       int pend_a = -1, pend_b = -1;
@@ -284,12 +344,18 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
           mbar_wait(bar_full_b + 8 * sb, pb);
           const uint32_t b_addr = b_ring + sb * (uint32_t)P.b_stage_bytes;
 #pragma unroll
-          for (int j = 0; j < GT; ++j) {
+          for (int j = 0; j < (BLK ? 1 : GT); ++j) {
             if (j < ntile) {
               mbar_wait(bar_full_a + 8 * sa, pa);
+              const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
               if (!s_skip[sa]) {
                 wg_fence();
-                issue_stage<KG, TPG, NT>(acc[j], a_ring + sa * (uint32_t)P.a_stage_bytes, b_addr, a_pitch, P.tap_off);
+                if (!BLK) {
+                  issue_stage<KG, TPG, NT>(acc[j], a_addr, b_addr, a_pitch, a_sbo, P.tap_off);
+                } else {
+#pragma unroll
+                  for (int k = 0; k < GT; ++k) issue_stage<KG, TPG, NT>(acc[k], a_addr + boff[k], b_addr, a_pitch, a_sbo, P.tap_off);
+                }
                 wg_commit();
                 wg_wait<1>();
                 release(pend_a, bar_empty_a);
@@ -342,17 +408,32 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
       int b = (int)(v0 / ntile_total);
 #pragma unroll
       for (int j = 0; j < GT; ++j) {
-        if (j < ntile) {
-          const long long vj = v0 + j;
-          const int bj = (int)(vj / ntile_total), tj = (int)(vj - (long long)bj * ntile_total);
-          if (bj != b) { if (P.ssum) flush_stats(b); b = bj; }
-          const int p_lo = P.p_begin + tj * 128 + r_lo, p_hi = p_lo + 8;
-          const bool in_lo = p_lo < P.p_end, in_hi = p_hi < P.p_end;
-          bool ok_lo = in_lo, ok_hi = in_hi;
-          if (P.rp > 0) {
-            const int z0 = p_lo % P.rp, y0 = (p_lo / P.rp) % P.rp, z1 = p_hi % P.rp, y1 = (p_hi / P.rp) % P.rp;
-            ok_lo = ok_lo && z0 >= 1 && z0 <= P.rp - 2 && y0 >= 1 && y0 <= P.rp - 2;
-            ok_hi = ok_hi && z1 >= 1 && z1 <= P.rp - 2 && y1 >= 1 && y1 <= P.rp - 2;
+        if (j < (BLK ? nbw : ntile)) {
+          int tj = 0, p_lo, p_hi;
+          bool ok_lo, ok_hi;
+          bool in_lo, in_hi;
+          if (!BLK) {
+            const long long vj = v0 + j;
+            const int bj = (int)(vj / ntile_total);
+            tj = (int)(vj - (long long)bj * ntile_total);
+            if (bj != b) { if (P.ssum) flush_stats(b); b = bj; }
+            p_lo = P.p_begin + tj * 128 + r_lo; p_hi = p_lo + 8;
+            in_lo = p_lo < P.p_end; in_hi = p_hi < P.p_end;
+            ok_lo = in_lo; ok_hi = in_hi;
+            if (TPG != 1) {                               // 3x3x3 row tiles: halo rows are stored as zeros
+              const int z0 = p_lo % P.rp, y0 = (p_lo / P.rp) % P.rp, z1 = p_hi % P.rp, y1 = (p_hi / P.rp) % P.rp;
+              ok_lo = ok_lo && z0 >= 1 && z0 <= P.rp - 2 && y0 >= 1 && y0 <= P.rp - 2;
+              ok_hi = ok_hi && z1 >= 1 && z1 <= P.rp - 2 && y1 >= 1 && y1 <= P.rp - 2;
+            }
+          } else {
+            // fragment row i of block k is voxel (y0 + i / 8, z0 + i % 8): this thread's rows are y-lines y0 + 2 wq
+            // and y0 + 2 wq + 1 at z0 + lane / 4.  Rows past r (a last block of an r that is not a multiple of 8) are
+            // neither stored nor counted.
+            const int k = g_f + 2 * j + wg, x = k / P.npl, rem = k - x * P.npl, yb = rem / P.nzb, zb = rem - yb * P.nzb;
+            const int y = 1 + 8 * yb + 2 * wq, z = 1 + 8 * zb + (lane >> 2);
+            p_lo = ((x + 1) * P.rp + y) * P.rp + z; p_hi = p_lo + P.rp;
+            ok_lo = y <= P.r && z <= P.r; ok_hi = y + 1 <= P.r && z <= P.r;
+            in_lo = ok_lo; in_hi = ok_hi;
           }
 #pragma unroll
           for (int i = 0; i < NT / 8; ++i) {
@@ -413,6 +494,73 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
       }
       if (P.ssum) flush_stats(b);
     }
+  }
+}
+
+// GroupNorm statistics of a 3x3x3 output computed on interior blocks, in exactly the grouping of the 128-row-tile
+// epilogue above (same items, warps, shuffle trees and fp32 partial sums; halo rows count as zeros), read back from the
+// stored output.  The fp32 partials of the two groupings round differently, and the denoising loop amplifies a one-ulp
+// change of an AdaGN scale over its 1000 steps; this pass keeps the statistics -- and so every output -- identical.
+template <int NT>
+__global__ void __launch_bounds__(256) k_conv_stats(Params P) {
+  constexpr int GT = tiles_per_item(NT);
+  __shared__ float s_stat[CONSUMER_WARPS * 2 * NT];
+  const int tid = threadIdx.x, cw = tid >> 5, lane = tid & 31, wg = cw >> 2, wq = cw & 3, et = tid;
+  for (int i = tid; i < CONSUMER_WARPS * 2 * NT; i += 256) s_stat[i] = 0.0f;
+  __syncthreads();
+  const int r_lo = 64 * wg + 16 * wq + (lane >> 2), c_lo = 2 * (lane & 3);
+  const int ntile_total = P.ntile;
+  const long long U = (long long)(P.cout_pad / NT) * P.B * ntile_total;
+  Items items = make_items(U, ntile_total, P.B, P.G, P.sched);
+  int nt, ntile;
+  long long v0;
+  while (items.next(nt, v0, ntile)) {
+    const int n0 = nt * NT;
+    auto flush_stats = [&](int bb) {
+      __syncthreads();
+      if (et < NT) {
+        float s = 0.f, qq = 0.f;
+#pragma unroll
+        for (int w = 0; w < CONSUMER_WARPS; ++w) {
+          s += s_stat[(w * 2 + 0) * NT + et]; qq += s_stat[(w * 2 + 1) * NT + et];
+          s_stat[(w * 2 + 0) * NT + et] = 0.0f; s_stat[(w * 2 + 1) * NT + et] = 0.0f;
+        }
+        atomicAdd(P.ssum + (size_t)bb * P.cout_pad + n0 + et, (double)s);
+        atomicAdd(P.ssq + (size_t)bb * P.cout_pad + n0 + et, (double)qq);
+      }
+      __syncthreads();
+    };
+    int b = (int)(v0 / ntile_total);
+#pragma unroll
+    for (int j = 0; j < GT; ++j) {
+      if (j < ntile) {
+        const long long vj = v0 + j;
+        const int bj = (int)(vj / ntile_total), tj = (int)(vj - (long long)bj * ntile_total);
+        if (bj != b) { flush_stats(b); b = bj; }
+        const int p_lo = P.p_begin + tj * 128 + r_lo, p_hi = p_lo + 8;
+        const int z0 = p_lo % P.rp, y0 = (p_lo / P.rp) % P.rp, z1 = p_hi % P.rp, y1 = (p_hi / P.rp) % P.rp;
+        const bool ok_lo = p_lo < P.p_end && z0 >= 1 && z0 <= P.rp - 2 && y0 >= 1 && y0 <= P.rp - 2;
+        const bool ok_hi = p_hi < P.p_end && z1 >= 1 && z1 <= P.rp - 2 && y1 >= 1 && y1 <= P.rp - 2;
+#pragma unroll 4
+        for (int i = 0; i < NT / 8; ++i) {
+          const int col = 8 * i + c_lo, ch = n0 + col, g = ch >> 2;
+          float2 lo = make_float2(0.f, 0.f), hi = lo;
+          if (g < P.Gout_store) {
+            const float* o = reinterpret_cast<const float*>(P.out + ((size_t)b * P.Gout_store + g) * P.rows) + (ch & 3);
+            if (ok_lo) lo = *reinterpret_cast<const float2*>(o + (size_t)p_lo * 4);
+            if (ok_hi) hi = *reinterpret_cast<const float2*>(o + (size_t)p_hi * 4);
+          }
+          const float x0 = lo.x, x1 = lo.y, x2 = hi.x, x3 = hi.y;
+          const float s0 = red8<0>(x0 + x2), s1 = red8<0>(x1 + x3);
+          const float q0 = red8<0>(fmaf(x0, x0, x2 * x2)), q1 = red8<0>(fmaf(x1, x1, x3 * x3));
+          if (lane < 4) {
+            float* st = s_stat + (cw * 2) * NT + col;
+            st[0] += s0; st[1] += s1; st[NT] += q0; st[NT + 1] += q1;
+          }
+        }
+      }
+    }
+    flush_stats(b);
   }
 }
 
@@ -504,25 +652,67 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   tc_shape(w, NT, KG, nchunk, ntg, tpg);
   P.in = in; P.w = w.tc.w; P.bias = w.bias; P.out = out; P.ssum = ssum; P.ssq = ssq;
   P.Gin = Gin; P.Gout_store = Gout_store; P.cout_pad = w.cout_pad;
-  P.rows = geo.rows; P.p_begin = geo.p_begin; P.p_end = geo.p_end; P.rp = geo.rp;
+  P.rows = geo.rows; P.p_begin = geo.p_begin; P.p_end = geo.p_end;
   P.ntg = ntg; P.tpg = tpg; P.KG = KG; P.nchunk = nchunk; P.NT = NT;
+  P.b_stage_bytes = tpg * KG * NT * 16;
+  P.B = B;
+  P.occ = geo.occ; P.occ_stride = geo.occ_stride;
+  const size_t fixed = tc::smem_fixed(NT, tpg);
+  // 3x3x3 with N = 128 runs on interior blocks (BLK); its chunking (16 channels) and so every output's accumulation
+  // order are those of the row tiles.  N <= 64 keeps the 128-row tiles: its 32-channel chunks leave no room for a
+  // block group's window beside the two weight slabs, and 16-channel chunks would reorder every output's sums.
+  const bool blk = w.ntaps == 27 && NT == 128;
+  // the 128-row tiles of [p_begin, p_end): the work space of row-tile kernels, and of the statistics pass (k_conv_stats)
+  const int ntile_rows = cdiv(geo.p_end - geo.p_begin, 128);
+  int ntile;
+  P.halo = 0;
   if (w.ntaps == 27) {
-    int rp = geo.rp;
+    const int rp = geo.rp, r = rp - 2;
     for (int dx = 0; dx < 3; ++dx) P.tg_off[dx] = (dx - 1) * rp * rp;
     for (int dy = 0; dy < 3; ++dy) for (int dz = 0; dz < 3; ++dz) P.tap_off[dy * 3 + dz] = (dy - 1) * rp + (dz - 1);
-    P.halo = rp + 1;
+    P.r = r; P.rp = rp;
   } else {
-    P.tg_off[0] = 0; P.tap_off[0] = 0; P.halo = 0;
+    P.tg_off[0] = 0; P.tap_off[0] = 0;
   }
-  P.stage_rows = 128 + 2 * P.halo;
+  if (blk) {
+    const int rp = P.rp, r = P.r;
+    P.nzb = cdiv(r, 8); P.npl = P.nzb * P.nzb; P.nblk = r * P.npl;
+    // Blocks per group: two per accumulator set (one per warpgroup).  A group's window is its blocks' rows plus every
+    // tap's neighbours: from (y0-1, z0-1) of its first block to (y0+8, z0+8) of its last; the largest sets the stage.
+    // At N = 128 that is two whole x-planes at r = 8 (200 rows) and 8 y-lines x 16 z at r = 16 (180 rows).
+    const int ib = 2 * tc::tiles_per_item(NT);
+    int wrows = 0;
+    for (int f = 0; f < P.nblk; f += ib) {
+      const int l = std::min(f + ib, P.nblk) - 1;
+      wrows = std::max(wrows, tc::block_row(l, rp, P.nzb, P.npl) - tc::block_row(f, rp, P.nzb, P.npl) + 9 * rp + 10);
+    }
+    P.ib = ib;
+    P.stage_rows = wrows;
+    ntile = cdiv(P.nblk, ib);
+    P.G = 1;
+  } else {
+    if (w.ntaps == 27) P.halo = P.rp + 1;
+    P.stage_rows = 128 + 2 * P.halo;
+    ntile = ntile_rows;
+    // row tiles per work item: as many as the accumulator registers hold (the weight slab of a stage is then shared by
+    // that many MMA groups); parallelism does not depend on G -- the kernel cuts the flat tile space into equal ranges per CTA
+    P.G = tc::tiles_per_item(NT);
+  }
+  P.ntile = ntile;
   P.a_stage_bytes = KG * P.stage_rows * 16;
-  P.b_stage_bytes = tpg * KG * NT * 16;
-  int ntile = cdiv(geo.p_end - geo.p_begin, 128);
+  // The weight ring.  A block group takes one A stage per weight slab, so the copies run ahead of the tensor cores by
+  // as many slabs as the weight ring holds: deepen it to 3-4 while at least 4 A stages (and one per slab) still fit --
+  // under the side-stream cap when one is set.  Row tiles share a slab among up to 4 tiles and keep 2.
+  int b_stages = 2;
+  if (blk) {
+    const long long limit = (c->conv_smem_cap > 0 ? c->conv_smem_cap : 227LL * 1024) - (long long)fixed;
+    while (b_stages < tc::MAX_B_STAGES &&
+           (limit - (long long)(b_stages + 1) * P.b_stage_bytes) / P.a_stage_bytes >= std::max(4, b_stages + 1))
+      ++b_stages;
+  }
+  P.b_stages = b_stages;
+  const long long a_room = 227LL * 1024 - (long long)fixed - (long long)b_stages * P.b_stage_bytes;
   int n_tiles_n = w.cout_pad / NT;
-  // row tiles per work item: as many as the accumulator registers hold (the weight slab of a stage is then shared by
-  // that many MMA groups); parallelism does not depend on G -- the kernel cuts the flat tile space into equal ranges per CTA
-  P.G = tc::tiles_per_item(NT);
-  P.B = B;
   // Round-based items (sched 1) for 3x3x3 grids whose input is well beyond the L2: the three x-plane sweeps of a tile then
   // hit the L2 instead of re-reading DRAM.  Measured on an H100 SXM (400 W, B = 32, kernel alone, sched 0 / 1 alternated
   // twice): every grid above 1.6x the 50 MB L2 runs faster with rounds (64 ch @ 32^3, 322 MB: 7-9 %; 32 ch @ 32^3,
@@ -530,10 +720,7 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   // (one pair of runs of one 25 MB grid excepted), and one contiguous range per CTA is kept.
   const double in_bytes = (double)B * Gin * geo.rows * 16.0;
   P.sched = w.ntaps == 27 && in_bytes > 1.6 * c->l2_bytes ? 1 : 0;
-  P.occ = geo.occ; P.occ_stride = geo.occ_stride;
-  const size_t fixed = tc::smem_fixed(NT, tpg);
-  long long room = 227LL * 1024 - (long long)fixed - (long long)tc::B_STAGES * P.b_stage_bytes;
-  int a_stages = (int)(room / P.a_stage_bytes);
+  int a_stages = (int)(a_room / P.a_stage_bytes);
   // Sharing an SM with the side stream.  FPS and the neighbour searches run on the side stream during the first
   // ~1 ms of a step (32 CTAs x <= 26 KB of shared memory, latency-bound); a persistent convolution CTA that claims all
   // 227 KB cannot become resident on their SMs, and with the static item split the whole convolution then takes two
@@ -541,31 +728,48 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   // flags side-stream work (Ctx::conv_smem_cap) the ring gives up a slot or two -- never below 4 -- and the side
   // kernels opt into the maximum shared-memory carve-out, because an SM only hosts kernels of one carve-out at a time.
   if (c->conv_smem_cap > 0 && a_stages >= 5) {
-    int capped = (int)(((long long)c->conv_smem_cap - (long long)fixed - (long long)tc::B_STAGES * P.b_stage_bytes) / P.a_stage_bytes);
+    int capped = (int)(((long long)c->conv_smem_cap - (long long)fixed - (long long)b_stages * P.b_stage_bytes) / P.a_stage_bytes);
     if (capped >= 4 && capped < a_stages) a_stages = capped;
   }
   if (a_stages > tc::MAX_A_STAGES) a_stages = tc::MAX_A_STAGES;
   if (a_stages < 2) { set_error("conv_tc: shared memory cannot hold the operand pipeline (N=%d, KG=%d)", NT, KG); return LION_ERR_ARG; }
   P.a_stages = a_stages;
-  size_t smem = (size_t)a_stages * P.a_stage_bytes + (size_t)tc::B_STAGES * P.b_stage_bytes + fixed;
+  size_t smem = (size_t)a_stages * P.a_stage_bytes + (size_t)b_stages * P.b_stage_bytes + fixed;
   if (smem > 227 * 1024) { set_error("conv_tc: %zu bytes of shared memory needed", smem); return LION_ERR_ARG; }
   // persistent, at most one CTA per SM: the fewest CTAs that still reach the minimal maximum of tiles per CTA
-  // (224 tiles on 132 SMs: 112 CTAs x 2 tiles, not 132 CTAs x 1-2 -- every CTA streams the whole weight tensor from L2,
-  // and the r = 8 layers are bound by exactly that)
-  long long n_units = (long long)ntile * n_tiles_n * B;
-  long long per_cta = (n_units + c->num_sms - 1) / c->num_sms;
-  int grid = (int)((n_units + per_cta - 1) / per_cta);
-#define CONV_TC_CASE(kg, tpg_, nt_)                                                                       \
-  if (KG == kg && tpg == tpg_ && NT == nt_) {                                                             \
+  // (224 tiles on 132 SMs: 112 CTAs x 2 tiles, not 132 CTAs x 1-2 -- every CTA streams the whole weight tensor from L2
+  // once per item, and the r = 8 layers are bound by exactly that)
+  auto grid_for = [&](int nt_per_shape) {
+    long long n_units = (long long)nt_per_shape * n_tiles_n * B;
+    long long per_cta = (n_units + c->num_sms - 1) / c->num_sms;
+    return (int)((n_units + per_cta - 1) / per_cta);
+  };
+  const int grid = grid_for(ntile);
+  // block groups: the GroupNorm statistics come from k_conv_stats, over the row tiles' items
+  tc::Params S = P;
+  if (blk && ssum) {
+    P.ssum = nullptr; P.ssq = nullptr;
+    S.ntile = ntile_rows; S.G = tc::tiles_per_item(NT);
+  }
+  auto stats = [&]() -> int {
+    if (!(blk && ssum)) return 0;
+    LION_LAUNCH(c, tc::k_conv_stats<128>, grid_for(ntile_rows), 256, 0, S);
+    return check_launch(c, "conv_tc stats");
+  };
+#define CONV_TC_CASE(kg, tpg_, nt_, blk_)                                                                 \
+  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_) {                                              \
     static DevOnce attr_once;                                                                             \
     if (attr_once.need()) {                                                                               \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
     }                                                                                                     \
-    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_>), grid, tc::THREADS, smem, P);                           \
-    return check_launch(c, "conv_tc");                                                                    \
+    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_>), grid, tc::THREADS, smem, P);                     \
+    LION_TRY(check_launch(c, "conv_tc"));                                                                 \
+    return stats();                                                                                       \
   }
-#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32) CONV_TC_CASE(kg, tpg_, 64) CONV_TC_CASE(kg, tpg_, 96) CONV_TC_CASE(kg, tpg_, 128)
+#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false) CONV_TC_CASE(kg, tpg_, 64, false) CONV_TC_CASE(kg, tpg_, 96, false)
   CONV_TC_NT(2, 1) CONV_TC_NT(4, 1) CONV_TC_NT(8, 1) CONV_TC_NT(2, 9) CONV_TC_NT(4, 9) CONV_TC_NT(8, 9)
+  CONV_TC_CASE(2, 1, 128, false) CONV_TC_CASE(4, 1, 128, false) CONV_TC_CASE(8, 1, 128, false)
+  CONV_TC_CASE(2, 9, 128, true) CONV_TC_CASE(4, 9, 128, true)
 #undef CONV_TC_NT
 #undef CONV_TC_CASE
   set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps", NT, KG, tpg);

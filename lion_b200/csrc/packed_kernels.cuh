@@ -306,8 +306,10 @@ __global__ void k_scatter(const float4* __restrict__ feat, const int* __restrict
 // Correctness scaffold and small-shape fallback; the tensor-core kernel (conv_tc.cu) has the
 // same contract:
 //   out[b][co/4][p] = bias + sum_taps sum_ci W[tap][ci][co] * in[b][ci/4][p + off[tap]]
-//   for p in [p_begin, p_end); rows whose (y,z) lie in the halo are written as zeros and
-//   excluded from the statistics;  ssum/ssq[b][co] += sum / sum of squares over valid rows.
+//   for the interior rows p of [p_begin, p_end);  ssum/ssq[b][co] += sum / sum of squares over them.
+//   Rows whose (y,z) lie in the halo are not part of the result: this kernel writes them as zeros, the
+//   tensor-core kernel leaves them unwritten, so readers of a 3x3x3 output (k_act_grid, k_devox_fuse,
+//   k_vg_to_cm) read interior rows only.
 // ------------------------------------------------------------------------------------
 // ConvGeom: model.cuh
 
