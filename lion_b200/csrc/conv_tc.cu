@@ -27,7 +27,8 @@
 //   * Output contract: rows of [p_begin, p_end) are written (halo rows as zeros), except on interior blocks, which
 //     leave the halo rows as they were: every consumer of a 3x3x3 output reads interior rows only.  Each output's
 //     accumulation order is the row tiles' (same channel chunks, x-planes, taps, k-steps), and the GroupNorm sums of
-//     interior blocks come from k_conv_stats in the row tiles' grouping: results are identical either way.
+//     interior blocks come from k_conv_stats, which re-reads the output and sums it over the row tiles' items with the
+//     epilogue's statistics routine (halo_mask, stat_add, stat_flush): results are identical either way.
 //   * persistent CTAs (one per SM, 288 threads): warps 0-7 = two consumer warpgroups (wgmma into
 //     registers, then the epilogue: +bias -> row mask -> coalesced float4 stores, GroupNorm sum /
 //     sum-of-squares per warp in shared memory, one fp64 atomic per channel per shape and item),
@@ -86,8 +87,6 @@ struct Params {
   // monotonic and Swish is quasi-convex (one minimum), so max_i swish(s*x_i + t) = max(swish(s*min + t), swish(s*max + t)):
   // the consumer needs 2 of the 32 values.
   float* pool_mm;
-  // row-major output (the y = x W GEMM of the sparse first convolution): out_rm[(b*rows + p) * ld_rm + n], no PF store
-  float* out_rm; int ld_rm;
   int sched;             // work distribution: 0 contiguous range per CTA, 1 interleaved items (see k_conv_tc)
 };
 
@@ -160,6 +159,45 @@ __device__ __forceinline__ Items make_items(long long U, int ntile_total, int B,
     it.big = (int)(u_end - u_begin) > q; it.k = 0;
   }
   return it;
+}
+
+// GroupNorm statistics in the row tiles' grouping, shared by k_conv_tc's epilogue and k_conv_stats so that both sum
+// alike: per fragment a shuffle tree over the warp's 8 row pairs, per-warp fp32 partials in s_stat [8 consumer warps]
+// [sum, sum of squares][NT], and per (shape, item) a fixed-order sum over the warps with one fp64 atomic per channel.
+//
+// 3x3x3 row tiles: rows p_lo and p_lo + 8 of a fragment that are y / z halo rows of their x plane count as zeros.
+__device__ __forceinline__ void halo_mask(int p_lo, int rp, bool& ok_lo, bool& ok_hi) {
+  const int p_hi = p_lo + 8;
+  const int z0 = p_lo % rp, y0 = (p_lo / rp) % rp, z1 = p_hi % rp, y1 = (p_hi / rp) % rp;
+  ok_lo = ok_lo && z0 >= 1 && z0 <= rp - 2 && y0 >= 1 && y0 <= rp - 2;
+  ok_hi = ok_hi && z1 >= 1 && z1 <= rp - 2 && y1 >= 1 && y1 <= rp - 2;
+}
+// adds one fragment -- channels col, col + 1 of rows p_lo (x0, x1) and p_lo + 8 (x2, x3) -- to consumer warp cw's partials
+template <int NT>
+__device__ __forceinline__ void stat_add(float* s_stat, int cw, int lane, int col, float x0, float x1, float x2, float x3) {
+  const float s0 = red8<0>(x0 + x2), s1 = red8<0>(x1 + x3);
+  const float q0 = red8<0>(fmaf(x0, x0, x2 * x2)), q1 = red8<0>(fmaf(x1, x1, x3 * x3));
+  if (lane < 4) {
+    float* st = s_stat + (cw * 2) * NT + col;
+    st[0] += s0; st[1] += s1; st[NT] += q0; st[NT + 1] += q1;
+  }
+}
+// moves the partials of shape b, channels n0 .. n0 + NT - 1 into ssum / ssq and zeroes them.  Named barrier 1 over the
+// 256 consumer threads (k_conv_tc's producer warp never gets here): every one of them must call it.
+template <int NT>
+__device__ __forceinline__ void stat_flush(const Params& P, float* s_stat, int et, int b, int n0) {
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  if (et < NT) {
+    float s = 0.f, qq = 0.f;
+#pragma unroll
+    for (int w = 0; w < CONSUMER_WARPS; ++w) {
+      s += s_stat[(w * 2 + 0) * NT + et]; qq += s_stat[(w * 2 + 1) * NT + et];
+      s_stat[(w * 2 + 0) * NT + et] = 0.0f; s_stat[(w * 2 + 1) * NT + et] = 0.0f;
+    }
+    atomicAdd(P.ssum + (size_t)b * P.cout_pad + n0 + et, (double)s);
+    atomicAdd(P.ssq + (size_t)b * P.cout_pad + n0 + et, (double)qq);
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
 }
 
 // BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), otherwise 128-row tiles
@@ -390,21 +428,6 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
       if (et < NT) s_bias[et] = P.bias ? P.bias[n0 + et] : 0.0f;
       asm volatile("bar.sync 1, 256;" ::: "memory");
       // GroupNorm statistics are per shape: flushed whenever the item moves on to the next shape, and at its end
-      // (per-warp partials -> fixed-order sum -> one fp64 atomic per channel; block-uniform control flow: bar.sync inside)
-      auto flush_stats = [&](int bb) {
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (et < NT) {
-          float s = 0.f, qq = 0.f;
-#pragma unroll
-          for (int w = 0; w < CONSUMER_WARPS; ++w) {
-            s += s_stat[(w * 2 + 0) * NT + et]; qq += s_stat[(w * 2 + 1) * NT + et];
-            s_stat[(w * 2 + 0) * NT + et] = 0.0f; s_stat[(w * 2 + 1) * NT + et] = 0.0f;
-          }
-          atomicAdd(P.ssum + (size_t)bb * P.cout_pad + n0 + et, (double)s);
-          atomicAdd(P.ssq + (size_t)bb * P.cout_pad + n0 + et, (double)qq);
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      };
       int b = (int)(v0 / ntile_total);
 #pragma unroll
       for (int j = 0; j < GT; ++j) {
@@ -416,15 +439,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
             const long long vj = v0 + j;
             const int bj = (int)(vj / ntile_total);
             tj = (int)(vj - (long long)bj * ntile_total);
-            if (bj != b) { if (P.ssum) flush_stats(b); b = bj; }
+            if (bj != b) { if (P.ssum) stat_flush<NT>(P, s_stat, et, b, n0); b = bj; }
             p_lo = P.p_begin + tj * 128 + r_lo; p_hi = p_lo + 8;
             in_lo = p_lo < P.p_end; in_hi = p_hi < P.p_end;
             ok_lo = in_lo; ok_hi = in_hi;
-            if (TPG != 1) {                               // 3x3x3 row tiles: halo rows are stored as zeros
-              const int z0 = p_lo % P.rp, y0 = (p_lo / P.rp) % P.rp, z1 = p_hi % P.rp, y1 = (p_hi / P.rp) % P.rp;
-              ok_lo = ok_lo && z0 >= 1 && z0 <= P.rp - 2 && y0 >= 1 && y0 <= P.rp - 2;
-              ok_hi = ok_hi && z1 >= 1 && z1 <= P.rp - 2 && y1 >= 1 && y1 <= P.rp - 2;
-            }
+            if (TPG != 1) halo_mask(p_lo, P.rp, ok_lo, ok_hi);   // halo rows are stored as zeros
           } else {
             // fragment row i of block k is voxel (y0 + i / 8, z0 + i % 8): this thread's rows are y-lines y0 + 2 wq
             // and y0 + 2 wq + 1 at z0 + lane / 4.  Rows past r (a last block of an r that is not a multiple of 8) are
@@ -440,26 +459,13 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
             const int col = 8 * i + c_lo;
             const float x0 = ok_lo ? acc[j][4 * i + 0] + s_bias[col] : 0.0f, x1 = ok_lo ? acc[j][4 * i + 1] + s_bias[col + 1] : 0.0f;
             const float x2 = ok_hi ? acc[j][4 * i + 2] + s_bias[col] : 0.0f, x3 = ok_hi ? acc[j][4 * i + 3] + s_bias[col + 1] : 0.0f;
-            if (P.ssum) {
-              const float s0 = red8<0>(x0 + x2), s1 = red8<0>(x1 + x3);
-              const float q0 = red8<0>(fmaf(x0, x0, x2 * x2)), q1 = red8<0>(fmaf(x1, x1, x3 * x3));
-              if (lane < 4) {
-                float* st = s_stat + (cw * 2) * NT + col;
-                st[0] += s0; st[1] += s1; st[NT] += q0; st[NT + 1] += q1;
-              }
-            }
+            if (P.ssum) stat_add<NT>(s_stat, cw, lane, col, x0, x1, x2, x3);
             if (TPG == 1 && P.pool_mm) {                 // all rows valid (rows % 128 == 0)
               const float mn0 = red8<1>(fminf(x0, x2)), mn1 = red8<1>(fminf(x1, x3));
               const float mx0 = red8<2>(fmaxf(x0, x2)), mx1 = red8<2>(fmaxf(x1, x3));
               if (lane < 4) {
                 float* sp = s_pool + (cw * 2) * NT + col;
                 sp[0] = mn0; sp[1] = mn1; sp[NT] = mx0; sp[NT + 1] = mx1;
-              }
-            } else if (TPG == 1 && P.out_rm) {
-              if (n0 + 8 * i < P.ld_rm) {
-                float* d = P.out_rm + n0 + col;
-                if (in_lo) *reinterpret_cast<float2*>(d + ((size_t)b * P.rows + p_lo) * P.ld_rm) = make_float2(x0, x1);
-                if (in_hi) *reinterpret_cast<float2*>(d + ((size_t)b * P.rows + p_hi) * P.ld_rm) = make_float2(x2, x3);
               }
             } else {
               // lanes 2k, 2k+1 hold channels 0-1 / 2-3 of a 4-channel group: swap halves so that each stores one float4
@@ -492,15 +498,15 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
           }
         }
       }
-      if (P.ssum) flush_stats(b);
+      if (P.ssum) stat_flush<NT>(P, s_stat, et, b, n0);
     }
   }
 }
 
-// GroupNorm statistics of a 3x3x3 output computed on interior blocks, in exactly the grouping of the 128-row-tile
-// epilogue above (same items, warps, shuffle trees and fp32 partial sums; halo rows count as zeros), read back from the
-// stored output.  The fp32 partials of the two groupings round differently, and the denoising loop amplifies a one-ulp
-// change of an AdaGN scale over its 1000 steps; this pass keeps the statistics -- and so every output -- identical.
+// GroupNorm statistics of a 3x3x3 output computed on interior blocks, read back from the stored output and summed by
+// the row tiles' items and warps through the epilogue's own routine (halo_mask, stat_add, stat_flush).  The fp32
+// partials of a different grouping would round differently, and the denoising loop amplifies a one-ulp change of an
+// AdaGN scale over its 1000 steps; this pass keeps the statistics -- and so every output -- identical to the row tiles'.
 template <int NT>
 __global__ void __launch_bounds__(256) k_conv_stats(Params P) {
   constexpr int GT = tiles_per_item(NT);
@@ -516,31 +522,16 @@ __global__ void __launch_bounds__(256) k_conv_stats(Params P) {
   long long v0;
   while (items.next(nt, v0, ntile)) {
     const int n0 = nt * NT;
-    auto flush_stats = [&](int bb) {
-      __syncthreads();
-      if (et < NT) {
-        float s = 0.f, qq = 0.f;
-#pragma unroll
-        for (int w = 0; w < CONSUMER_WARPS; ++w) {
-          s += s_stat[(w * 2 + 0) * NT + et]; qq += s_stat[(w * 2 + 1) * NT + et];
-          s_stat[(w * 2 + 0) * NT + et] = 0.0f; s_stat[(w * 2 + 1) * NT + et] = 0.0f;
-        }
-        atomicAdd(P.ssum + (size_t)bb * P.cout_pad + n0 + et, (double)s);
-        atomicAdd(P.ssq + (size_t)bb * P.cout_pad + n0 + et, (double)qq);
-      }
-      __syncthreads();
-    };
     int b = (int)(v0 / ntile_total);
 #pragma unroll
     for (int j = 0; j < GT; ++j) {
       if (j < ntile) {
         const long long vj = v0 + j;
         const int bj = (int)(vj / ntile_total), tj = (int)(vj - (long long)bj * ntile_total);
-        if (bj != b) { flush_stats(b); b = bj; }
+        if (bj != b) { stat_flush<NT>(P, s_stat, et, b, n0); b = bj; }
         const int p_lo = P.p_begin + tj * 128 + r_lo, p_hi = p_lo + 8;
-        const int z0 = p_lo % P.rp, y0 = (p_lo / P.rp) % P.rp, z1 = p_hi % P.rp, y1 = (p_hi / P.rp) % P.rp;
-        const bool ok_lo = p_lo < P.p_end && z0 >= 1 && z0 <= P.rp - 2 && y0 >= 1 && y0 <= P.rp - 2;
-        const bool ok_hi = p_hi < P.p_end && z1 >= 1 && z1 <= P.rp - 2 && y1 >= 1 && y1 <= P.rp - 2;
+        bool ok_lo = p_lo < P.p_end, ok_hi = p_hi < P.p_end;
+        halo_mask(p_lo, P.rp, ok_lo, ok_hi);
 #pragma unroll 4
         for (int i = 0; i < NT / 8; ++i) {
           const int col = 8 * i + c_lo, ch = n0 + col, g = ch >> 2;
@@ -550,17 +541,11 @@ __global__ void __launch_bounds__(256) k_conv_stats(Params P) {
             if (ok_lo) lo = *reinterpret_cast<const float2*>(o + (size_t)p_lo * 4);
             if (ok_hi) hi = *reinterpret_cast<const float2*>(o + (size_t)p_hi * 4);
           }
-          const float x0 = lo.x, x1 = lo.y, x2 = hi.x, x3 = hi.y;
-          const float s0 = red8<0>(x0 + x2), s1 = red8<0>(x1 + x3);
-          const float q0 = red8<0>(fmaf(x0, x0, x2 * x2)), q1 = red8<0>(fmaf(x1, x1, x3 * x3));
-          if (lane < 4) {
-            float* st = s_stat + (cw * 2) * NT + col;
-            st[0] += s0; st[1] += s1; st[NT] += q0; st[NT + 1] += q1;
-          }
+          stat_add<NT>(s_stat, cw, lane, col, lo.x, lo.y, hi.x, hi.y);
         }
       }
     }
-    flush_stats(b);
+    stat_flush<NT>(P, s_stat, et, b, n0);
   }
 }
 
@@ -590,44 +575,31 @@ __global__ void k_pack_tc(const float* __restrict__ wt, float* __restrict__ w, i
 
 }  // namespace tc
 
-static void tc_shape(const ConvW& w, int& NT, int& KG, int& nchunk, int& ntg, int& tpg) {
-  NT = w.cout_pad < 128 ? w.cout_pad : 128;
-  ntg = w.ntaps == 27 ? 3 : 1;
-  tpg = w.ntaps == 27 ? 9 : 1;
-  int G = w.cin_pad / 4;
-  // 3x3x3: 32-channel chunks (36 wgmmas per activation stage) for N <= 64 -- the per-stage barrier
-  // round trip is amortised over more MMAs -- and 16-channel chunks for N = 128, where the 9-tap
-  // weight slab (2 x 72 KB) leaves room for a 16-channel ring only.
-  // 1x1: 32-channel chunks.
-  if (w.ntaps == 27) KG = (NT > 64) ? 4 : 8;
-  else KG = 8;
-  if (G < KG) KG = (G <= 2) ? 2 : ((G <= 4) ? 4 : 8);
-  nchunk = (G + KG - 1) / KG;
-}
-
+// The tiling of a convolution: decided here once, stored in w.tc with the packing laid out for it, and read by
+// conv_tc_run, ygemm and sa_fused.  Adds the step that packs w.wt into w.tc.w.
 int conv_tc_prepare(Model* m, ConvW& w) {
   w.tc = ConvTcW();
   if (!(w.ntaps == 27 || w.ntaps == 1)) return 0;
   if (w.cout_pad < 32 || w.cout_pad % 32) return 0;      // the kernel is instantiated for N = 32, 64, 96, 128
-  int NT, KG, nchunk, ntg, tpg;
-  tc_shape(w, NT, KG, nchunk, ntg, tpg);
-  if (w.cout_pad % NT) return 0;
-  size_t total = (size_t)(w.cout_pad / NT) * nchunk * ntg * tpg * KG * NT * 4;
-  LION_TRY(m->dmalloc(&w.tc.w, total));
-  w.tc.ck = KG * 4; w.tc.nchunk = nchunk; w.tc.n = NT;
-  PackJob j{2, w.wt, nullptr, w.tc.w, w.ntaps, w.cin_pad, w.cout_pad, NT, 0};
-  j.kmap = nullptr;
-  m->jobs.push_back(j);
-  return 0;
-}
-
-int conv_tc_pack_job(const PackJob& j) {
-  ConvW tmp;
-  tmp.ntaps = j.a; tmp.cin_pad = j.b; tmp.cout_pad = j.c;
-  int NT, KG, nchunk, ntg, tpg;
-  tc_shape(tmp, NT, KG, nchunk, ntg, tpg);
-  size_t total = (size_t)(j.c / NT) * nchunk * ntg * tpg * KG * NT * 4;
-  tc::k_pack_tc<<<(unsigned)cdivz(total, 256), 256>>>(j.src, j.dst, j.a, j.b, j.c, NT, nchunk, ntg, tpg, KG);
+  ConvTcW t;
+  t.NT = w.cout_pad < 128 ? w.cout_pad : 128;
+  if (w.cout_pad % t.NT) return 0;
+  t.ntg = w.ntaps == 27 ? 3 : 1;
+  t.tpg = w.ntaps == 27 ? 9 : 1;
+  const int G = w.cin_pad / 4;
+  // 3x3x3: 32-channel chunks (36 wgmmas per activation stage) for N <= 64 -- the per-stage barrier
+  // round trip is amortised over more MMAs -- and 16-channel chunks for N = 128, where the 9-tap
+  // weight slab (2 x 72 KB) leaves room for a 16-channel ring only.
+  // 1x1: 32-channel chunks.
+  t.KG = (w.ntaps == 27 && t.NT > 64) ? 4 : 8;
+  if (G < t.KG) t.KG = (G <= 2) ? 2 : ((G <= 4) ? 4 : 8);
+  t.nchunk = (G + t.KG - 1) / t.KG;
+  const size_t total = (size_t)(w.cout_pad / t.NT) * t.nchunk * t.ntg * t.tpg * t.KG * t.NT * 4;
+  LION_TRY(m->dmalloc(&t.w, total));
+  w.tc = t;
+  m->repack.push_back([t, wt = w.wt, ntaps = w.ntaps, cin_pad = w.cin_pad, cout_pad = w.cout_pad, total] {
+    tc::k_pack_tc<<<(unsigned)cdivz(total, 256), 256>>>(wt, t.w, ntaps, cin_pad, cout_pad, t.NT, t.nchunk, t.ntg, t.tpg, t.KG);
+  });
   return 0;
 }
 
@@ -638,22 +610,17 @@ bool conv_tc_usable(const ConvW& w, const ConvGeom& geo) {
 }
 
 int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, double* ssum, double* ssq,
-                const ConvGeom& geo, int B, float* pool_mm, float* out_rm, int ld_rm) {
+                const ConvGeom& geo, int B, float* pool_mm) {
   tc::Params P{};
-  if (out_rm && (w.ntaps != 1 || w.cout_pad < 128 || ld_rm % 16)) {
-    set_error("conv_tc: the row-major epilogue needs a 1x1 convolution with >= 128 output channels"); return LION_ERR_ARG;
-  }
-  P.out_rm = out_rm; P.ld_rm = ld_rm;
   if (pool_mm && (w.ntaps != 1 || geo.p_begin != 0 || geo.p_end != geo.rows || geo.rows % 128)) {
     set_error("conv_tc: the pooled epilogue needs a 1x1 convolution over a multiple of 128 rows"); return LION_ERR_ARG;
   }
   P.pool_mm = pool_mm;
-  int NT, KG, nchunk, ntg, tpg;
-  tc_shape(w, NT, KG, nchunk, ntg, tpg);
+  const int NT = w.tc.NT, KG = w.tc.KG, tpg = w.tc.tpg;
   P.in = in; P.w = w.tc.w; P.bias = w.bias; P.out = out; P.ssum = ssum; P.ssq = ssq;
   P.Gin = Gin; P.Gout_store = Gout_store; P.cout_pad = w.cout_pad;
   P.rows = geo.rows; P.p_begin = geo.p_begin; P.p_end = geo.p_end;
-  P.ntg = ntg; P.tpg = tpg; P.KG = KG; P.nchunk = nchunk; P.NT = NT;
+  P.ntg = w.tc.ntg; P.tpg = tpg; P.KG = KG; P.nchunk = w.tc.nchunk; P.NT = NT;
   P.b_stage_bytes = tpg * KG * NT * 16;
   P.B = B;
   P.occ = geo.occ; P.occ_stride = geo.occ_stride;

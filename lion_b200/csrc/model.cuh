@@ -1,5 +1,6 @@
 // lion_b200 -- host-side model description shared by net.cu, conv_tc.cu and global_prior.cu.
 #pragma once
+#include <functional>
 #include <memory>
 #include <vector>
 #include "common.cuh"
@@ -8,12 +9,14 @@ namespace lion {
 
 struct StyleLayer { const float* w; const float* b; int n_out; int out_off; };
 
-// tensor-core packing of a convolution's weights (conv_tc.cu); w == nullptr -> SIMT kernel only
+// tensor-core packing of a convolution's weights and the tiling it is packed for (conv_tc_prepare);
+// w == nullptr -> SIMT kernel only
 struct ConvTcW {
-  float* w = nullptr;
-  int ck = 0;        // input channels per pipeline chunk (8, 16 or 32)
-  int nchunk = 0;
-  int n = 0;         // wgmma N (= padded output channels, <= 128)
+  float* w = nullptr;    // [n-tile][chunk][tap group][tap][KG][NT][4], tf32-rounded
+  int NT = 0;            // output channels per CTA (wgmma N, <= 128)
+  int KG = 0;            // 4-channel input groups per pipeline chunk (2, 4 or 8)
+  int nchunk = 0;        // chunks
+  int ntg = 0, tpg = 0;  // tap groups (x planes) and taps per group: (3, 9) or (1, 1)
 };
 
 struct Cursor {
@@ -28,9 +31,6 @@ struct Cursor {
 
 struct ConvW {
   int ntaps = 1, cin_ref = 0, cin_pad = 0, cout = 0, cout_pad = 0;
-  const float* w_ref = nullptr;
-  const float* b_ref = nullptr;
-  int* d_kmap = nullptr;
   float* wt = nullptr;      // [ntaps][cin_pad][cout_pad]   (SIMT kernel)
   float* bias = nullptr;    // [cout_pad]
   ConvTcW tc;               // tensor-core packing (conv_tc.cuh); tc.w == nullptr when unsupported
@@ -105,8 +105,6 @@ int global_prior_build(Model* m, Cursor& cur);
 int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B);
 void global_prior_free(GlobalPriorBlk*);
 
-struct PackJob { int type; const float* src; const int* kmap; float* dst; int a, b, c, d, e; };
-
 struct Model {
   Ctx* ctx = nullptr;
   int kind = 0;
@@ -114,7 +112,10 @@ struct Model {
   std::vector<const float*> params;
   std::vector<void*> owned;
   std::vector<cudaEvent_t> events;
-  std::vector<PackJob> jobs;
+  // Launches that derive the packed weights from the parameters, in order (a step may read an earlier one's output).
+  // Run once at build and again by lion_model_refresh after the parameters changed in place.  A step captures device
+  // pointers and sizes by value: the ConvWs it serves live in vectors that may still grow while the model is built.
+  std::vector<std::function<void()>> repack;
   std::vector<StyleLayer> style_layers;
   StyleLayer* d_style_layers = nullptr;
   int style_total = 0;
@@ -153,7 +154,7 @@ struct Model {
 };
 
 
-int make_conv(Model* m, ConvW& w, const float* w_ref, const float* b_ref, int ntaps, int cin_ref, int cout,
+int make_conv(Model* m, ConvW& w, const float* w_src, const float* b_src, int ntaps, int cin_ref, int cout,
               const std::vector<int>& kmap);
 std::vector<int> ident_map(int c);
 static inline int roundup(int a, int b) { return (a + b - 1) / b * b; }
@@ -171,7 +172,6 @@ struct ConvGeom {
 
 // conv_tc.cu
 int conv_tc_prepare(Model* m, ConvW& w);
-int conv_tc_pack_job(const PackJob& j);
 bool conv_tc_usable(const ConvW& w, const ConvGeom& geo);
 // sparse first convolution, GEMM half (sparse_conv.cu)
 bool ygemm_usable(const ConvW& y);
@@ -182,6 +182,6 @@ int sa_fused_run(Ctx* c, const SABlk& s, const float4* feat, const float4* point
                  const float* scale1, const float* shift1, double* ssum, double* ssq, int stat_stride, float* pool_mm,
                  int B, int N);
 int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, double* ssum,
-                double* ssq, const ConvGeom& geo, int B, float* pool_mm = nullptr, float* out_rm = nullptr, int ld_rm = 0);
+                double* ssq, const ConvGeom& geo, int B, float* pool_mm = nullptr);
 
 }  // namespace lion

@@ -85,7 +85,7 @@ int ctx_reserve_zgrid(Ctx* c, size_t bytes) {
 }
 
 // weight packing kernels
-__global__ void k_pack_conv_w(const float* __restrict__ w_ref, const int* __restrict__ kmap, float* __restrict__ wt,
+__global__ void k_pack_conv_w(const float* __restrict__ w_src, const int* __restrict__ kmap, float* __restrict__ wt,
                               int ntaps, int cin_ref, int cin_pad, int cout, int cout_pad) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   size_t total = (size_t)ntaps * cin_pad * cout_pad;
@@ -95,7 +95,7 @@ __global__ void k_pack_conv_w(const float* __restrict__ w_ref, const int* __rest
   int t = i / ((size_t)cout_pad * cin_pad);
   int src = kmap[ci];
   float v = 0.0f;
-  if (src >= 0 && co < cout) v = w_ref[((size_t)co * cin_ref + src) * ntaps + t];
+  if (src >= 0 && co < cout) v = w_src[((size_t)co * cin_ref + src) * ntaps + t];
   wt[i] = v;
 }
 // sparse first convolution: the 27 taps side by side, wy[ci][t * cout_pad + co] = wt[t][ci][co] (zero beyond 27 * cout_pad)
@@ -113,23 +113,27 @@ __global__ void k_pad_vec(const float* __restrict__ src, float* __restrict__ dst
 
 
 // build a conv's packed forms. kmap: packed input channel -> reference input channel (-1 = zero)
-int make_conv(Model* m, ConvW& w, const float* w_ref, const float* b_ref, int ntaps, int cin_ref, int cout,
+int make_conv(Model* m, ConvW& w, const float* w_src, const float* b_src, int ntaps, int cin_ref, int cout,
               const std::vector<int>& kmap) {
   w.ntaps = ntaps; w.cin_ref = cin_ref; w.cin_pad = (int)kmap.size(); w.cout = cout;
   w.cout_pad = (cout <= 4) ? 4 : roundup(cout, 8);
-  w.w_ref = w_ref; w.b_ref = b_ref;
-  if (!w_ref) { set_error("model parameters exhausted while building a convolution"); return LION_ERR_ARG; }
+  if (!w_src) { set_error("model parameters exhausted while building a convolution"); return LION_ERR_ARG; }
   if (w.cin_pad % 4) { set_error("packed input channels must be a multiple of 4 (got %d)", w.cin_pad); return LION_ERR_ARG; }
-  LION_TRY(m->dmalloc(&w.d_kmap, kmap.size()));
-  LION_CHECK_CUDA(cudaMemcpy(w.d_kmap, kmap.data(), kmap.size() * sizeof(int), cudaMemcpyHostToDevice));
-  size_t nw = (size_t)ntaps * w.cin_pad * w.cout_pad;
+  int* kmap_dev = nullptr;
+  LION_TRY(m->dmalloc(&kmap_dev, kmap.size()));
+  LION_CHECK_CUDA(cudaMemcpy(kmap_dev, kmap.data(), kmap.size() * sizeof(int), cudaMemcpyHostToDevice));
+  const size_t nw = (size_t)ntaps * w.cin_pad * w.cout_pad;
   LION_TRY(m->dmalloc(&w.wt, nw));
-  m->jobs.push_back({0, w_ref, w.d_kmap, w.wt, ntaps, cin_ref, w.cin_pad, cout, w.cout_pad});
-  if (b_ref) {
+  m->repack.push_back([w_src, kmap_dev, wt = w.wt, ntaps, cin_ref, cin_pad = w.cin_pad, cout, cout_pad = w.cout_pad, nw] {
+    k_pack_conv_w<<<(unsigned)cdivz(nw, 256), 256>>>(w_src, kmap_dev, wt, ntaps, cin_ref, cin_pad, cout, cout_pad);
+  });
+  if (b_src) {
     LION_TRY(m->dmalloc(&w.bias, (size_t)w.cout_pad));
-    m->jobs.push_back({1, b_ref, nullptr, w.bias, cout, w.cout_pad, 0, 0, 0});
+    m->repack.push_back([b_src, bias = w.bias, cout, cout_pad = w.cout_pad] {
+      k_pad_vec<<<cdiv(cout_pad, 128), 128>>>(b_src, bias, cout, cout_pad);
+    });
   }
-  LION_TRY(conv_tc_prepare(m, w));     // optional tensor-core packing (adds its own job)
+  LION_TRY(conv_tc_prepare(m, w));     // optional tensor-core packing (adds its own step)
   return 0;
 }
 std::vector<int> ident_map(int c) {
@@ -138,19 +142,8 @@ std::vector<int> ident_map(int c) {
   return k;
 }
 
-int run_jobs(Model* m) {
-  for (auto& j : m->jobs) {
-    if (j.type == 0) {
-      size_t total = (size_t)j.a * j.c * j.e;
-      k_pack_conv_w<<<(unsigned)cdivz(total, 256), 256>>>(j.src, j.kmap, j.dst, j.a, j.b, j.c, j.d, j.e);
-    } else if (j.type == 1) {
-      k_pad_vec<<<cdiv(j.b, 128), 128>>>(j.src, j.dst, j.a, j.b);
-    } else if (j.type == 3) {
-      k_pack_taps_wide<<<(unsigned)cdivz((size_t)j.a * j.c, 256), 256>>>(j.src, j.dst, j.a, j.b, j.c);
-    } else {
-      LION_TRY(conv_tc_pack_job(j));
-    }
-  }
+int run_repack(Model* m) {
+  for (auto& step : m->repack) step();
   LION_CHECK_CUDA(cudaGetLastError());
   LION_CHECK_CUDA(cudaDeviceSynchronize());
   return 0;
@@ -207,8 +200,10 @@ int make_pvconv(Model* m, PVConvBlk& p, Cursor& cur, int cin, int cout, int r, b
     y.ntaps = 1; y.cin_ref = p.c1.cin_pad; y.cin_pad = p.c1.cin_pad;
     y.cout = y.cout_pad = roundup(27 * p.c1.cout_pad, 128);
     LION_TRY(m->dmalloc(&y.wt, (size_t)y.cin_pad * y.cout_pad));
-    m->jobs.push_back({3, p.c1.wt, nullptr, y.wt, y.cin_pad, p.c1.cout_pad, y.cout_pad, 0, 0});
-    LION_TRY(conv_tc_prepare(m, y));
+    m->repack.push_back([wt = p.c1.wt, wy = y.wt, cin_pad = y.cin_pad, cout_pad = p.c1.cout_pad, ny_pad = y.cout_pad] {
+      k_pack_taps_wide<<<(unsigned)cdivz((size_t)cin_pad * ny_pad, 256), 256>>>(wt, wy, cin_pad, cout_pad, ny_pad);
+    });
+    LION_TRY(conv_tc_prepare(m, y));     // packs y.wt: its step must follow the one above
   }
   LION_TRY(make_adagn(m, p.g1, cur, cout, plain));
   const float* w2 = cur.next(); const float* b2 = cur.next();
@@ -308,11 +303,11 @@ static ConvGeom geom_grid(int r) {
 
 // out rows in [p_begin,p_end) of every (b, group < Gout_store); statistics optional
 static int run_conv(Fwd& f, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store,
-                    double* ssum, double* ssq, const ConvGeom& geo, float* pool_mm = nullptr, float* out_rm = nullptr, int ld_rm = 0) {
+                    double* ssum, double* ssq, const ConvGeom& geo, float* pool_mm = nullptr) {
   if (Gin * 4 != w.cin_pad) { set_error("conv: input has %d channels, weights expect %d", Gin * 4, w.cin_pad); return LION_ERR_ARG; }
   if (conv_tc_usable(w, geo))
-    return conv_tc_run(f.c, w, in, Gin, out, Gout_store, ssum, ssq, geo, f.B, pool_mm, out_rm, ld_rm);
-  if (pool_mm || out_rm) { set_error("conv: the pooled epilogue exists on the tensor-core path only"); return LION_ERR_STATE; }
+    return conv_tc_run(f.c, w, in, Gin, out, Gout_store, ssum, ssq, geo, f.B, pool_mm);
+  if (pool_mm) { set_error("conv: the pooled epilogue exists on the tensor-core path only"); return LION_ERR_STATE; }
   int span = geo.p_end - geo.p_begin;
   if (w.cout_pad == 4) {
     LION_LAUNCH(f.c, k_conv_simt<4>, dim3(cdiv(span, 128), 1, f.B), 128, geo.ntaps * 16 * sizeof(float),
@@ -1218,7 +1213,7 @@ extern "C" int lion_model_create(LionCtx* ctx, int kind, const int* desc, int nd
     LION_TRY(m->dmalloc(&m->d_style_layers, m->style_layers.size()));
     LION_CHECK_CUDA(cudaMemcpy(m->d_style_layers, m->style_layers.data(), m->style_layers.size() * sizeof(StyleLayer), cudaMemcpyHostToDevice));
   }
-  LION_TRY(run_jobs(m));
+  LION_TRY(run_repack(m));
   *out = h.release();
   return 0;
 }
@@ -1226,7 +1221,7 @@ extern "C" int lion_model_destroy(LionModel* h) { delete h; return 0; }
 extern "C" int lion_model_refresh(LionModel* h) {
   LION_REQUIRE(h, "lion_model_refresh: null model");
   LION_CHECK_CUDA(cudaSetDevice(h->m.ctx->device));
-  return run_jobs(&h->m);
+  return run_repack(&h->m);
 }
 
 extern "C" int lion_unet_forward(LionModel* h, const float* x, const float* t, const float* style, const float* clip,
@@ -1485,7 +1480,7 @@ extern "C" int lion_bench_conv(LionCtx* ctx, int ntaps, int cin, int cout, int r
   k_fill_pattern<<<cdiv(cout, 256), 256>>>(bref, cout, 0.1f);
   ConvW w;
   LION_TRY(make_conv(m, w, wref, bref, ntaps, cin, cout, ident_map(cin)));
-  LION_TRY(run_jobs(m));
+  LION_TRY(run_repack(m));
   ConvGeom geo = ntaps == 27 ? geom_grid(r_or_rows) : geom_rows(r_or_rows);
   size_t guard = ntaps == 27 ? (size_t)(r_or_rows + 2) * (r_or_rows + 2) + (r_or_rows + 2) + 8 : 256;
   size_t n_in = (size_t)B * (cin / 4) * geo.rows + 2 * guard, n_out = (size_t)B * (cout / 4) * geo.rows + 2 * guard;

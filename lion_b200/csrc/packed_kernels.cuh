@@ -160,7 +160,7 @@ __global__ void k_scatter_compact(const float4* __restrict__ feat, const int* __
 }
 
 // Sparse first convolution of a PVConv, second half.  y[b][v][t][c] = W[t]^T x[v] for every occupied voxel v and tap t
-// (one dense GEMM over the compact list, conv_tc.cu with a row-major epilogue); here every interior output voxel p sums,
+// (one dense GEMM over the compact list, k_ygemm in sparse_conv.cu); here every interior output voxel p sums,
 // in ascending tap order, the rows y[vgrid[p + off(t)]][t] of its occupied neighbours -- each y row is read exactly
 // once -- adds the bias, stores the raw convolution output and accumulates the GroupNorm statistics.  Deterministic.
 //   one warp = 32 consecutive interior voxels; accumulators [32][C] in shared memory; C <= 64 (2 channels per lane)

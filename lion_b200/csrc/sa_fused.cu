@@ -207,7 +207,7 @@ bool sa_fused_usable(const SABlk& s) {
   if (s.mlp.conv.size() != 2 || s.k != 32 || s.m % 4) return false;
   const ConvW &c1 = s.mlp.conv[0], &c2 = s.mlp.conv[1];
   if (!c1.tc.w || !c2.tc.w || c1.cout != c1.cout_pad || c2.cout != c2.cout_pad) return false;
-  return s.cfeat == 32 && c1.cout == 32 && c2.cout == 64 && c1.tc.n == 32 && c2.tc.n == 64 && c1.tc.ck == 32 && c2.tc.ck == 32;
+  return s.cfeat == 32 && c1.cout == 32 && c2.cout == 64 && c1.tc.NT == 32 && c2.tc.NT == 64 && c1.tc.KG == 8 && c2.tc.KG == 8;
 }
 
 // pass 1 (scale1 == nullptr): layer-1 statistics; pass 2: layer-2 statistics + pooled min / max

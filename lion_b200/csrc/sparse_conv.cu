@@ -111,8 +111,8 @@ __global__ void __launch_bounds__(256, 2) k_ygemm(Params P) {
 }  // namespace spc
 
 bool ygemm_usable(const ConvW& y) {
-  return y.tc.w && y.ntaps == 1 && y.tc.n == 128 && y.cin_pad % 8 == 0 && y.cin_pad <= 128 &&
-         y.tc.nchunk * (y.tc.ck / 4) == y.cin_pad / 4;
+  return y.tc.w && y.ntaps == 1 && y.tc.NT == 128 && y.cin_pad % 8 == 0 && y.cin_pad <= 128 &&
+         y.tc.nchunk * y.tc.KG == y.cin_pad / 4;
 }
 
 // y[b][v][0..ld) = x[b][v][:] * Wy for the first nocc[b] rows of every shape
@@ -120,7 +120,7 @@ int ygemm_run(Ctx* c, const ConvW& y, const float4* xc, float* out, int ld, cons
   if (ld % 32) { set_error("ygemm: row pitch %d is not a multiple of 32", ld); return LION_ERR_ARG; }
   spc::Params P{};
   P.x = xc; P.w = y.tc.w; P.y = out; P.nocc = nocc;
-  P.G = y.tc.nchunk * (y.tc.ck / 4);        // group slots of the packing (>= cin_pad / 4; extra slots hold zero weights)
+  P.G = y.tc.nchunk * y.tc.KG;              // group slots of the packing (>= cin_pad / 4; extra slots hold zero weights)
   if (P.G != y.cin_pad / 4) { set_error("ygemm: packed groups %d != input groups %d", P.G, y.cin_pad / 4); return LION_ERR_STATE; }
   P.N = N; P.B = B; P.ld = ld;
   P.blocks_per_shape = (N + spc::ROWS - 1) / spc::ROWS;
