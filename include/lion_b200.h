@@ -256,6 +256,18 @@ int lion_emd_approx_saved(const float* xyz1, const float* xyz2, float* cost, flo
 int lion_emd_backward(const float* xyz1, const float* xyz2, const float* ratios, const float* grad_cost,
                       float* grad1, float* grad2, int B, int N, int M, void* stream);
 
+/* Occupancy grid of the JSD score (utils/evaluation_metrics_fast.py:604-647, entropy_of_occupancy_grid).
+ * clouds [S,N,3] point-major, cells [K,3] (the cell centres, any order) -> for every cell c
+ *   point_counts[c] = number of points, over all clouds, whose nearest cell is c   (the reference's grid_counters)
+ *   cloud_counts[c] = number of clouds with at least one point whose nearest cell is c   (grid_bernoulli_rvars)
+ * Both outputs are overwritten (zeroed on `stream` first).  The nearest cell minimises the exact float64 squared
+ * distance (dx*dx + dy*dy) + dz*dz of the float32 inputs, every operation rounded separately (no contraction); on an
+ * exact tie the lowest cell index wins.  Integer atomics only: the counts are deterministic.  Brute force over the
+ * cells (no pruning), so points anywhere -- also far outside the cell table -- get their exact nearest cell.
+ * Requires S, N, K > 0, S * N <= INT_MAX and K <= 1,572,864 cells (the per-cloud bitmap lives in shared memory). */
+int lion_occupancy_grid(const float* clouds, const float* cells, int S, int N, int K, int* point_counts,
+                        int* cloud_counts, void* stream);
+
 /* measurement hook (bench.py roofline leg): average device time of `iters` launches of the
  * convolution kernel alone (CUDA events on `stream`), on synthetic data: ntaps = 27 -> 3x3x3
  * over [B, cin, r^3] (r_or_rows = r), ntaps = 1 -> 1x1 over r_or_rows rows.  flops_out = the

@@ -9,7 +9,8 @@ host-side mirror of the reference's Python interface for that path:
     lion_b200.models.lion                       LION (demo wrapper; diffusers-style scheduler restated)
     lion_b200.third_party.ChamferDistancePytorch.chamfer3D.dist_chamfer_3D   Chamfer NN (metrics)
     lion_b200.third_party.PyTorchEMD.emd_nograd / .emd                       approximate EMD (metrics)
-    lion_b200.utils.evaluation_metrics_fast     pairwise CD / EMD matrices (not aliased: the reference module holds more)
+    lion_b200.utils.evaluation_metrics_fast     pairwise CD / EMD matrices, MMD / COV / 1-NNA and JSD scores
+    lion_b200.utils.eval_helper / .data_helper  compute_score of a sample file, normalize_point_clouds
     lion_b200.trainers.train_2prior             generate_samples_vada_2prior (DDPM, DDIM and ODE routes)
     lion_b200.trainers.train_prior              Trainer.sample / Trainer.eval_sample (sampling-side Trainer)
     lion_b200.models.pvcnn2 / .shapelatent_modules / .distributions          VAE encoder path (non-Ada blocks)

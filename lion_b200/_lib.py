@@ -80,6 +80,7 @@ def _proto(lib):
         "lion_emd_approx_saved": (P(vp, vp, vp, vp, i, i, i, vp), i),
         "lion_emd_backward": (P(vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_emd_pairwise": (P(vp, vp, vp, i, i, i, i, vp), i),
+        "lion_occupancy_grid": (P(vp, vp, i, i, i, vp, vp, vp), i),
         "lion_bench_conv": (P(vp, i, i, i, i, i, i, i, C.POINTER(f), C.POINTER(C.c_double), vp), i),
     }
     for name, (args, res) in sig.items():

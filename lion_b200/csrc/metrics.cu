@@ -17,6 +17,8 @@
 // a candidate costs 3 LDS + Q x 8 FP32/select instructions; the pairwise kernel handles both
 // directions of one (sample, reference) pair per CTA and reduces the two means in a fixed order
 // (deterministic, no atomics, no [Nr, N, 3] expansion of the sample cloud).
+#include <climits>
+#include <math_constants.h>
 #include "common.cuh"
 #include "../../include/lion_b200.h"
 
@@ -539,4 +541,101 @@ extern "C" int lion_emd_pairwise(const float* samples, const float* refs, float*
   LION_REQUIRE(N <= EMD_MAX && M <= EMD_MAX, "lion_emd_pairwise: clouds of at most %d points (got %d, %d)", EMD_MAX, N, M);
   LION_REQUIRE((long long)n_sample * n_ref < (1LL << 31), "lion_emd_pairwise: too many pairs");
   return emd_launch<false>(samples, refs, out, nullptr, n_sample * n_ref, N, M, n_ref, 1, stream);
+}
+
+// =====================================================================================
+// occupancy grid of the JSD score (reference: utils/evaluation_metrics_fast.py:604-647,
+// entropy_of_occupancy_grid: sklearn NearestNeighbors over the grid cells, then per-point Python loops).
+//
+// One CTA per cloud.  Every thread keeps OCC_Q points in registers as doubles and scans the cell table, staged in
+// shared memory as double SoA in chunks of OCC_CHUNK cells, in index order with a strict `<`: the lowest cell index
+// wins an exact tie.  The squared distance is the exact float64 one, rounded op by op (no contraction), so the nearest
+// cell does not depend on the compiler.  A point adds 1 to point_counts[cell] and sets the cell's bit in the cloud's
+// bitmap in shared memory (K bits); once the whole cloud is done, every set bit adds 1 to cloud_counts[cell].  Integer
+// atomics only: the counts do not depend on the order the atomics land in.
+// =====================================================================================
+namespace lion {
+
+constexpr int OCC_THREADS = 256;
+constexpr int OCC_Q = 4;                        // points per thread and pass
+constexpr int OCC_CHUNK = 1024;                 // cells staged per pass (24 KB of doubles)
+constexpr int OCC_BITMAP_MAX = 192 * 1024;      // dynamic shared memory of the bitmap: K <= 1,572,864 cells
+
+__device__ __forceinline__ double occ_d2(double px, double py, double pz, double cx, double cy, double cz) {
+  const double dx = __dsub_rn(px, cx), dy = __dsub_rn(py, cy), dz = __dsub_rn(pz, cz);
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+__global__ void __launch_bounds__(OCC_THREADS)
+k_occupancy(const float* __restrict__ clouds, const float* __restrict__ cells, int n, int k_cells,
+            int* __restrict__ point_counts, int* __restrict__ cloud_counts) {
+  __shared__ double sx[OCC_CHUNK], sy[OCC_CHUNK], sz[OCC_CHUNK];
+  extern __shared__ unsigned bitmap[];           // [cdiv(k_cells, 32)]
+  const int words = (k_cells + 31) >> 5;
+  for (int w = threadIdx.x; w < words; w += OCC_THREADS) bitmap[w] = 0u;
+  const float* pc = clouds + (size_t)blockIdx.x * n * 3;
+  for (int p0 = 0; p0 < n; p0 += OCC_THREADS * OCC_Q) {
+    double px[OCC_Q], py[OCC_Q], pz[OCC_Q], best[OCC_Q];
+    int bi[OCC_Q];
+#pragma unroll
+    for (int u = 0; u < OCC_Q; ++u) {
+      const int j = p0 + u * OCC_THREADS + threadIdx.x;
+      const int jj = j < n ? j : 0;
+      px[u] = pc[jj * 3]; py[u] = pc[jj * 3 + 1]; pz[u] = pc[jj * 3 + 2];
+      best[u] = CUDART_INF; bi[u] = 0;
+    }
+    for (int k0 = 0; k0 < k_cells; k0 += OCC_CHUNK) {
+      const int kn = min(OCC_CHUNK, k_cells - k0);
+      __syncthreads();
+      for (int k = threadIdx.x; k < kn; k += OCC_THREADS) {
+        sx[k] = cells[(size_t)(k0 + k) * 3]; sy[k] = cells[(size_t)(k0 + k) * 3 + 1]; sz[k] = cells[(size_t)(k0 + k) * 3 + 2];
+      }
+      __syncthreads();
+#pragma unroll 2
+      for (int k = 0; k < kn; ++k) {
+        const double cx = sx[k], cy = sy[k], cz = sz[k];
+#pragma unroll
+        for (int u = 0; u < OCC_Q; ++u) {
+          const double d = occ_d2(px[u], py[u], pz[u], cx, cy, cz);
+          if (d < best[u]) { best[u] = d; bi[u] = k0 + k; }
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < OCC_Q; ++u) {
+      if (p0 + u * OCC_THREADS + threadIdx.x < n) {
+        atomicAdd(point_counts + bi[u], 1);
+        atomicOr(bitmap + (bi[u] >> 5), 1u << (bi[u] & 31));
+      }
+    }
+  }
+  __syncthreads();
+  for (int w = threadIdx.x; w < words; w += OCC_THREADS) {
+    unsigned bits = bitmap[w];
+    while (bits) {
+      const int b = __ffs(bits) - 1;
+      bits &= bits - 1;
+      atomicAdd(cloud_counts + (w << 5) + b, 1);
+    }
+  }
+}
+
+}  // namespace lion
+
+extern "C" int lion_occupancy_grid(const float* clouds, const float* cells, int S, int N, int K, int* point_counts,
+                                   int* cloud_counts, void* stream) {
+  LION_REQUIRE(clouds && cells && point_counts && cloud_counts && S > 0 && N > 0 && K > 0, "lion_occupancy_grid: bad arguments");
+  LION_REQUIRE((long long)S * N <= INT_MAX, "lion_occupancy_grid: S * N = %lld points exceed INT_MAX", (long long)S * N);
+  const size_t bitmap = (size_t)cdiv(K, 32) * sizeof(unsigned);
+  LION_REQUIRE(bitmap <= (size_t)OCC_BITMAP_MAX, "lion_occupancy_grid: at most %d cells (got %d)", OCC_BITMAP_MAX * 8, K);
+  Ctx c;
+  c.stream = (cudaStream_t)stream;
+  static DevOnce attr_once;
+  if (attr_once.need()) {
+    LION_CHECK_CUDA(cudaFuncSetAttribute(k_occupancy, cudaFuncAttributeMaxDynamicSharedMemorySize, OCC_BITMAP_MAX));
+  }
+  LION_TRY(memset_async(&c, point_counts, 0, (size_t)K * sizeof(int)));
+  LION_TRY(memset_async(&c, cloud_counts, 0, (size_t)K * sizeof(int)));
+  LION_LAUNCH(&c, k_occupancy, S, OCC_THREADS, bitmap, clouds, cells, N, K, point_counts, cloud_counts);
+  return check_launch(&c, "lion_occupancy_grid");
 }

@@ -77,8 +77,8 @@ class Trainer(object):
     def eval_sample(self, step=0, num_ref=None, batch_size_test=None, ddim_step=0, output_name=None, reference_seeding=False):
         """Generation half of base_trainer.eval_sample (:446-492): num_gen_iter batches of batch_size_test shapes per rank,
         re-seeded per batch, gathered over ranks; returns gen_pcs [num, N, 3] on the host (rank order) and saves them on
-        rank 0 when output_name is given.  The CD / EMD scores that follow in the reference are computed by
-        lion_b200.utils.evaluation_metrics_fast on request; MMD / COV / 1-NNA bookkeeping is out of scope."""
+        rank 0 when output_name is given.  The scores that follow in the reference (MMD / COV / 1-NNA, JSD) come from
+        lion_b200.utils.eval_helper.compute_score(output_name, ref_name)."""
         world = dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1
         rank = dist.get_rank() if world > 1 else 0
         batch_size_test = batch_size_test or self.cfg.data.batch_size_test
