@@ -532,17 +532,21 @@ __global__ void __launch_bounds__(256) k_conv_stats(Params P) {
         const int p_lo = P.p_begin + tj * 128 + r_lo, p_hi = p_lo + 8;
         bool ok_lo = p_lo < P.p_end, ok_hi = p_hi < P.p_end;
         halo_mask(p_lo, P.rp, ok_lo, ok_hi);
-#pragma unroll 4
+        // all of the tile's loads are issued before the first sum: the shuffles and shared-memory adds of stat_add would
+        // otherwise hold each load back behind the previous one's, one memory latency per channel group
+        float2 lo[NT / 8], hi[NT / 8];
+#pragma unroll
         for (int i = 0; i < NT / 8; ++i) {
-          const int col = 8 * i + c_lo, ch = n0 + col, g = ch >> 2;
-          float2 lo = make_float2(0.f, 0.f), hi = lo;
+          const int ch = n0 + 8 * i + c_lo, g = ch >> 2;
+          lo[i] = make_float2(0.f, 0.f); hi[i] = lo[i];
           if (g < P.Gout_store) {
             const float* o = reinterpret_cast<const float*>(P.out + ((size_t)b * P.Gout_store + g) * P.rows) + (ch & 3);
-            if (ok_lo) lo = *reinterpret_cast<const float2*>(o + (size_t)p_lo * 4);
-            if (ok_hi) hi = *reinterpret_cast<const float2*>(o + (size_t)p_hi * 4);
+            if (ok_lo) lo[i] = *reinterpret_cast<const float2*>(o + (size_t)p_lo * 4);
+            if (ok_hi) hi[i] = *reinterpret_cast<const float2*>(o + (size_t)p_hi * 4);
           }
-          stat_add<NT>(s_stat, cw, lane, col, lo.x, lo.y, hi.x, hi.y);
         }
+#pragma unroll
+        for (int i = 0; i < NT / 8; ++i) stat_add<NT>(s_stat, cw, lane, 8 * i + c_lo, lo[i].x, lo[i].y, hi[i].x, hi[i].y);
       }
     }
     stat_flush<NT>(P, s_stat, et, b, n0);

@@ -1,5 +1,8 @@
 """Time the convolution kernel alone on every shape of the PVCNN2 prior step (B=32):
-python tools/bench_convs.py  -> table + JSON lines (CUDA events via lion_bench_conv)."""
+python tools/bench_convs.py  -> table + JSON lines (CUDA events via lion_bench_conv).
+
+Next to each time: the operand bytes the launch moves from L2 into shared memory (operand_bytes) and the rate that
+makes -- the weight slabs every work item streams, and the activation windows of its tiles."""
 import ctypes as C
 import json
 import os
@@ -23,6 +26,65 @@ if ONLY:
     SHAPES = [s for s in SHAPES if s[5] == ONLY]
 if os.environ.get("TAPS"):           # TAPS=1 -> only the 1x1 shapes, TAPS=27 -> only the 3x3x3 ones
     SHAPES = [s for s in SHAPES if s[0] == int(os.environ["TAPS"])]
+
+
+def _tiles_per_item(nt):
+    return 4 if nt <= 32 else (2 if nt <= 64 else 1)
+
+
+def _block_row(k, rp, nzb, npl):
+    x, rem = divmod(k, npl)
+    yb, zb = divmod(rem, nzb)
+    return ((x + 1) * rp + 1 + 8 * yb) * rp + 1 + 8 * zb
+
+
+def operand_bytes(ntaps, cin, cout, r_or_rows, B, num_sms, l2_bytes):
+    """(work items, weight bytes, activation bytes) one launch of the tensor-core convolution reads from L2, from the
+    tiling of conv_tc_prepare / conv_tc_run (csrc/conv_tc.cu): every item streams its n-tile's nchunk x ntg weight slabs
+    once, and every tile the activation window of each slab.  Windows are counted whole: the clipped last window of a
+    shape and skipped all-zero windows of a sparse input are not subtracted."""
+    nt = cout if cout < 128 else 128
+    n_nt, kg_all = cout // nt, cin // 4
+    kg = 4 if (ntaps == 27 and nt > 64) else 8
+    if kg_all < kg:
+        kg = 2 if kg_all <= 2 else (4 if kg_all <= 4 else 8)
+    nchunk, ntg, tpg = -(-kg_all // kg), (3 if ntaps == 27 else 1), (9 if ntaps == 27 else 1)
+    b_stage = tpg * kg * nt * 16
+    if ntaps == 27 and nt == 128:                     # interior 8 x 8 blocks, groups of 2 per item
+        r, rp = r_or_rows, r_or_rows + 2
+        nzb = -(-r // 8)
+        npl, ib = nzb * nzb, 2
+        nblk = r * npl
+        stage_rows = max(_block_row(min(f + ib, nblk) - 1, rp, nzb, npl) - _block_row(f, rp, nzb, npl) + 9 * rp + 10
+                         for f in range(0, nblk, ib))
+        ntile, G, rows = -(-nblk // ib), 1, rp ** 3
+    else:                                             # 128-row tiles, up to G per item
+        rp = r_or_rows + 2 if ntaps == 27 else 0
+        rows = rp ** 3 if ntaps == 27 else r_or_rows
+        span = r_or_rows * rp * rp if ntaps == 27 else r_or_rows
+        stage_rows = 128 + (2 * (rp + 1) if ntaps == 27 else 0)
+        ntile, G = -(-span // 128), _tiles_per_item(nt)
+    U = n_nt * B * ntile
+    per_cta = -(-U // num_sms)
+    grid = -(-U // per_cta)
+    sched1 = ntaps == 27 and B * kg_all * rows * 16.0 > 1.6 * l2_bytes
+    q, n_p = divmod(U, grid)
+    m = -(-(q + (1 if n_p else 0)) // G)
+    items = 0
+    for i in range(grid):
+        u, u_end = U * i // grid, U * (i + 1) // grid
+        if sched1:                                    # one item per non-empty round (one n-tile: no cuts)
+            items += min(u_end - u, m)
+            continue
+        while u < u_end:                              # a contiguous range cut into evenly sized items per n-tile
+            run = min(u_end - u, B * ntile - u % (B * ntile))
+            k2 = -(-run // G)
+            u += -(-run // k2)
+            items += 1
+    slabs = nchunk * ntg
+    return items, items * slabs * b_stage, U * slabs * kg * stage_rows * 16
+
+
 torch.cuda.init()
 ITERS = int(os.environ.get("ITERS", "10"))      # ITERS=3000 CLOCKS=1: long enough for nvidia-smi to see the clock under load
 
@@ -38,6 +100,7 @@ def sample_clocks(stop, rows):
     p.terminate()
 
 
+props = torch.cuda.get_device_properties(0)
 tot = 0.0
 for nt, ci, co, r, n, label in SHAPES:
     ms, fl = C.c_float(), C.c_double()
@@ -50,8 +113,11 @@ for nt, ci, co, r, n, label in SHAPES:
     L.check(L.lib().lion_bench_conv(L.ctx(), nt, ci, co, r, B, ITERS, 2, C.byref(ms), C.byref(fl), L.stream()), label)
     tf = fl.value / (ms.value * 1e-3) / 1e12
     tot += ms.value * n
+    items, wb, ab = operand_bytes(nt, ci, co, r, B, props.multi_processor_count, props.L2_cache_size)
     rec = {"shape": label, "ntaps": nt, "cin": ci, "cout": co, "r_or_rows": r, "B": B, "ms": round(ms.value, 4),
-           "tflops_algorithmic": round(tf, 1), "launches_per_step": n}
+           "tflops_algorithmic": round(tf, 1), "launches_per_step": n, "items": items, "weight_gb": round(wb / 1e9, 3),
+           "activation_gb": round(ab / 1e9, 3), "weight_share": round(wb / (wb + ab), 2),
+           "l2_to_smem_gbs": round((wb + ab) / (ms.value * 1e-3) / 1e9)}
     if th is not None:
         stop.set()
         th.join(timeout=2)
