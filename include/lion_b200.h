@@ -24,6 +24,9 @@ int lion_ctx_create(int device, LionCtx** out);
 int lion_ctx_destroy(LionCtx* ctx);
 /* kernels launched by the last network-level call on this context (bench.py: gpu_launches) */
 int lion_ctx_last_launches(LionCtx* ctx);
+/* voxel blocks per work item of the last 128-channel 3x3x3 convolution on this context: 2, or 4 when there are enough
+ * groups to give every SM work (0 when the last convolution ran on 128-row tiles) */
+int lion_ctx_last_conv_group(LionCtx* ctx);
 /* Scratch-arena generation: bumped whenever a call had to re-allocate the per-device arena or zero grid.  A CUDA graph
  * captured on this context has the arena addresses baked in; it must not be replayed once the generation changed
  * (lion_b200._lib.capture_graph checks this and raises). */

@@ -31,6 +31,7 @@ def _proto(lib):
         "lion_ctx_create": (P(i, C.POINTER(vp)), i),
         "lion_ctx_destroy": (P(vp), i),
         "lion_ctx_last_launches": (P(vp), i),
+        "lion_ctx_last_conv_group": (P(vp), i),
         "lion_ctx_arena_bytes": (P(vp), sz),
         "lion_ctx_generation": (P(vp), C.c_uint),
         "lion_ctx_timeline": (P(vp, vp, vp, i), i),

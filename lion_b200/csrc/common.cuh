@@ -69,6 +69,8 @@ struct Ctx {
   // > 0 while side-stream kernels (FPS, neighbour searches) are expected in flight: persistent convolution CTAs then
   // leave this much shared memory unclaimed so that both can be resident on one SM (see conv_tc_run)
   int conv_smem_cap = 0;
+  // blocks per group of the last tensor-core convolution on interior blocks (2 or 4; 0 when it ran on row tiles)
+  int conv_group_blocks = 0;
   // LION_TIMELINE=1 (diagnostic, tools/timeline_step.py): %globaltimer stamps dropped into both streams at block
   // boundaries -- this image has no nsys, and a step's critical path across the two streams is not visible otherwise
   unsigned long long* d_stamps = nullptr;

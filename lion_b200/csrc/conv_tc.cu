@@ -11,7 +11,8 @@
 //     per wgmma.  Row tiles (1x1, and 3x3x3 with N <= 64): a block is 64 consecutive rows, two make a 128-row tile, and
 //     3x3x3 halo rows inside it are computed and stored as zeros.  Interior blocks (3x3x3 with N = 128): a block is
 //     8 y-lines x 8 z of one x-plane -- halo rows are neither computed nor written.  Blocks are ordered z fastest, then
-//     y, then x, and a group of 2 consecutive blocks of one shape is one work item.
+//     y, then x, and a group of 2 consecutive blocks of one shape is one work item -- 4 (two per warpgroup, twice the
+//     MMAs per weight slab and A stage) where B x ceil(blocks / 4) still gives every SM a group (conv_tc_run).
 //   * A operand: the activation tensor is [C/4][rows][4] in HBM, i.e. for 4 channels all rows
 //     are contiguous at a 16-byte pitch.  That *is* the canonical no-swizzle K-major wgmma
 //     layout (core matrix = 8 rows x 16 B = 128 contiguous bytes, SBO between 8-row groups,
@@ -22,8 +23,8 @@
 //     bytes viewed through a descriptor whose start address is shifted by (dy*(r+2)+dz) rows.  L2->SM traffic per
 //     MAC drops 9x versus reloading per tap.
 //   * B operand: weights pre-packed [n-tile][chunk][x-plane][tap][C/4][co][4] so one bulk copy
-//     brings the 9 taps of a (channel chunk, x-plane); a CTA reuses it for up to tiles_per_item
-//     blocks per warpgroup, whose accumulators all stay in registers (<= 128 per thread).
+//     brings the 9 taps of a (channel chunk, x-plane); a CTA reuses it for up to tiles_per_item row tiles or 2
+//     interior blocks per warpgroup, whose accumulators all stay in registers (<= 128 per thread).
 //   * Output contract: rows of [p_begin, p_end) are written (halo rows as zeros), except on interior blocks, which
 //     leave the halo rows as they were: every consumer of a 3x3x3 output reads interior rows only.  Each output's
 //     accumulation order is the row tiles' (same channel chunks, x-planes, taps, k-steps), and the GroupNorm sums of
@@ -32,7 +33,8 @@
 //   * persistent CTAs (one per SM, 288 threads): warps 0-7 = two consumer warpgroups (wgmma into
 //     registers, then the epilogue: +bias -> row mask -> coalesced float4 stores, GroupNorm sum /
 //     sum-of-squares per warp in shared memory, one fp64 atomic per channel per shape and item),
-//     warp 8 = bulk-copy producer.
+//     warp 8 = bulk-copy producer.  4-block groups run 384 threads: warps 8-11 give registers to the consumers (see
+//     conv_threads) and warp 8 alone copies.
 #include <algorithm>
 
 #include "common.cuh"
@@ -46,11 +48,19 @@ using namespace sm90;
 
 constexpr int CONSUMER_WARPS = 8;                    // two warpgroups: rows 0-63 / 64-127 of every tile
 constexpr int THREADS = 32 * CONSUMER_WARPS + 32;    // + warp 8, the producer
+// Two interior blocks per warpgroup need two 64-register accumulator sets per thread, more than the 168 registers a
+// thread of the 288-thread block gets (each of the SM's 4 register-file quarters holds 3 of its 9 warps).  Those kernels
+// run a whole producer warpgroup instead (384 threads, warp 8 copies, warps 9-11 exit) and move registers from it to
+// the consumers with setmaxnreg: one producer-warpgroup warp x 96 + two consumer warps x 200 registers per quarter,
+// 15,872 of 16,384 (ptxas: no spills; the consumers need about 180).
+__host__ __device__ constexpr int conv_threads(int BPW) { return BPW == 2 ? 32 * CONSUMER_WARPS + 128 : THREADS; }
+constexpr int PRODUCER_REGS = 96, CONSUMER_REGS = 200;
 constexpr int MAX_A_STAGES = 16;   // the A ring is as deep as shared memory allows (Params::a_stages)
 constexpr int MAX_B_STAGES = 4;   // the weight ring: 2 slabs, deeper for 3x3x3 where shared memory allows (Params::b_stages)
 constexpr int OCC_SMEM = 1024;       // bytes of per-item occupancy flags kept in shared memory (r <= 38)
 // row tiles per work item: their accumulators (NT / 2 registers per thread each, 64 in all) share one weight slab.  The
-// block's 288 threads get at most 168 registers each; more accumulators spill.
+// statistics pass (k_conv_stats) rebuilds the row tiles' GroupNorm grouping from it, so it must not change.  Interior
+// blocks have their own count per warpgroup (k_conv_tc's BPW, see conv_threads).
 __host__ __device__ constexpr int tiles_per_item(int NT) { return NT <= 32 ? 4 : (NT <= 64 ? 2 : 1); }
 // fixed shared memory after the A / B rings: bias, per-warp GroupNorm partials, the pooled epilogue's exchange (1x1 only),
 // barriers + flags, occupancy flags.  What the kernel does not use is left to the A ring.
@@ -96,18 +106,25 @@ __host__ __device__ __forceinline__ int block_row(int k, int rp, int nzb, int np
   return ((x + 1) * rp + 1 + 8 * yb) * rp + 1 + 8 * zb;
 }
 
-// all wgmmas of one (64-row block, channel chunk, tap group) for this warpgroup: TPG taps x KG/2 k-steps.  a_sbo is the
-// distance between the block's 8-row groups: 128 B for 64 consecutive rows, (r+2) * 16 B for 8 y-lines x 8 z.
-template <int KG, int TPG, int NT>
-__device__ __forceinline__ void issue_stage(float* d, uint32_t a_addr, uint32_t b_addr, uint32_t a_pitch, uint32_t a_sbo,
-                                            const int* tap_off) {
-  const uint64_t a0 = make_desc(a_addr, a_pitch, a_sbo), b0 = make_desc(b_addr, NT * 16, 128);
+// all wgmmas of NB 64-row blocks (operands at a_addr[0 .. NB-1]) for one (channel chunk, tap group) of this warpgroup:
+// TPG taps x KG/2 k-steps, the blocks interleaved per k-step (each accumulator set d[k] still takes its taps and k-steps
+// in order; the blocks share the weight descriptors).  a_sbo is the distance between a block's 8-row groups: 128 B for
+// 64 consecutive rows, (r+2) * 16 B for 8 y-lines x 8 z.
+template <int KG, int TPG, int NT, int NB = 1>
+__device__ __forceinline__ void issue_stage(float (*d)[NT / 2], const uint32_t* a_addr, uint32_t b_addr, uint32_t a_pitch,
+                                            uint32_t a_sbo, const int* tap_off) {
+  const uint64_t b0 = make_desc(b_addr, NT * 16, 128);
+  uint64_t a0[NB];
+#pragma unroll
+  for (int k = 0; k < NB; ++k) a0[k] = make_desc(a_addr[k], a_pitch, a_sbo);
 #pragma unroll
   for (int t = 0; t < TPG; ++t) {
-    const uint64_t at = a0 + (uint64_t)(int64_t)(TPG == 1 ? 0 : tap_off[t]);      // descriptor address unit = 16 B = 1 row
+    const uint64_t toff = (uint64_t)(int64_t)(TPG == 1 ? 0 : tap_off[t]);      // descriptor address unit = 16 B = 1 row
 #pragma unroll
     for (int ks = 0; ks < KG / 2; ++ks)
-      wgmma_tf32<NT>(d, at + (uint64_t)((ks * 2 * a_pitch) >> 4), b0 + (uint64_t)(((t * KG + ks * 2) * NT * 16) >> 4), 1);
+#pragma unroll
+      for (int k = 0; k < NB; ++k)
+        wgmma_tf32<NT>(d[k], a0[k] + toff + (uint64_t)((ks * 2 * a_pitch) >> 4), b0 + (uint64_t)(((t * KG + ks * 2) * NT * 16) >> 4), 1);
   }
 }
 
@@ -200,10 +217,13 @@ __device__ __forceinline__ void stat_flush(const Params& P, float* s_stat, int e
   asm volatile("bar.sync 1, 256;" ::: "memory");
 }
 
-// BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), otherwise 128-row tiles
-template <int KG, int TPG, int NT, bool BLK>
-__global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
-  constexpr int GT = tiles_per_item(NT);
+// BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), BPW of them per warpgroup and group (P.ib = 2 * BPW); otherwise
+// 128-row tiles
+template <int KG, int TPG, int NT, bool BLK, int BPW = 1>
+__global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
+  constexpr int GT = BLK ? BPW : tiles_per_item(NT);   // accumulator sets per thread
+  constexpr int NTHR = conv_threads(BPW);
+  constexpr bool SETREG = NTHR > THREADS;              // registers moved from the producer warpgroup to the consumers
   constexpr int NACC = NT / 2;                  // accumulator registers per thread and tile
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* sA = smem;
@@ -224,8 +244,8 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   // zero the A stages once: channel-group slots that a partial chunk does not load must hold
   // finite values (their weights are zero)
   if (P.Gin % KG != 0)
-    for (int i = tid; i < A_STAGES * P.a_stage_bytes / 16; i += THREADS) ((float4*)sA)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = tid; i < CONSUMER_WARPS * 2 * NT; i += THREADS) s_stat[i] = 0.0f;
+    for (int i = tid; i < A_STAGES * P.a_stage_bytes / 16; i += NTHR) ((float4*)sA)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = tid; i < CONSUMER_WARPS * 2 * NT; i += NTHR) s_stat[i] = 0.0f;
   if (tid == 0) {
     // a stage is released by every consumer warp once its wgmmas have read it
     for (int i = 0; i < A_STAGES; ++i) { mbar_init(bar_full_a + 8 * i, 1); mbar_init(bar_empty_a + 8 * i, CONSUMER_WARPS); }
@@ -255,8 +275,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   const long long U = (long long)n_nt * P.B * ntile_total;
   const Items items0 = make_items(U, ntile_total, P.B, P.G, P.sched);
 
-  if (warp == CONSUMER_WARPS) {
+  if (warp >= CONSUMER_WARPS) {
     // ===================== producer (whole warp; lane kg issues the copy of channel group kg) ====
+    if constexpr (SETREG) {
+      regs_dec<PRODUCER_REGS>();
+      if (warp > CONSUMER_WARPS) return;
+    }
     uint32_t sa = 0, pa = 0, sb = 0, pb = 0;          // ring positions and phase bits
     const uint32_t bytes = (uint32_t)P.stage_rows * 16u;
     const uint32_t sA_addr = smem_u32(sA), sB_addr = smem_u32(sB);
@@ -276,7 +300,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
           // the last sweep of an item is never skipped: every accumulator then receives at
           // least one (zero-initialising) MMA per item and needs no "was it touched" bookkeeping
           const bool may_skip = P.occ && !(cc == P.nchunk - 1 && tg == P.ntg - 1);
-          mbar_wait(bar_empty_b + 8 * sb, pb ^ 1);
+          mbar_wait<SETREG>(bar_empty_b + 8 * sb, pb ^ 1);
           if (lane == 0) {
             mbar_expect_tx(bar_full_b + 8 * sb, P.b_stage_bytes);
             bulk_g2s(sB_addr + sb * (uint32_t)P.b_stage_bytes, wsrc + (size_t)(cc * P.ntg + tg) * (P.b_stage_bytes / 4),
@@ -297,7 +321,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
               if (row0 + cnt > (long long)P.rows) cnt = (uint32_t)(P.rows - row0);
             }
             const float4* in_lane = P.in + ((size_t)bj * P.Gin + grp_lane) * P.rows;
-            mbar_wait(bar_empty_a + 8 * sa, pa ^ 1);
+            mbar_wait<SETREG>(bar_empty_a + 8 * sa, pa ^ 1);
             bool empty = false;
             if (may_skip) {
               // sparse input: the shape's occupancy flags (<= 1 KB) live in shared memory -- a broadcast LDS per
@@ -335,6 +359,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
   } else {
     // ===================== consumers ===========
     // row tiles: warpgroup wg computes rows 64 wg .. 64 wg + 63 of every tile.  Interior blocks: blocks wg, wg + 2, ...
+    if constexpr (SETREG) regs_inc<CONSUMER_REGS>();
     const int cw = warp, wg = cw >> 2, wq = cw & 3;
     const int et = tid;                                  // 0..255
     const uint32_t a_pitch = (uint32_t)P.stage_rows * 16u;
@@ -379,20 +404,22 @@ __global__ void __launch_bounds__(THREADS, 1) k_conv_tc(Params P) {
       int pend_a = -1, pend_b = -1;
       for (int cc = 0; cc < P.nchunk; ++cc) {
         for (int tg = 0; tg < P.ntg; ++tg) {
-          mbar_wait(bar_full_b + 8 * sb, pb);
+          mbar_wait<SETREG>(bar_full_b + 8 * sb, pb);
           const uint32_t b_addr = b_ring + sb * (uint32_t)P.b_stage_bytes;
 #pragma unroll
           for (int j = 0; j < (BLK ? 1 : GT); ++j) {
             if (j < ntile) {
-              mbar_wait(bar_full_a + 8 * sa, pa);
+              mbar_wait<SETREG>(bar_full_a + 8 * sa, pa);
               const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
               if (!s_skip[sa]) {
                 wg_fence();
                 if (!BLK) {
-                  issue_stage<KG, TPG, NT>(acc[j], a_addr, b_addr, a_pitch, a_sbo, P.tap_off);
+                  issue_stage<KG, TPG, NT>(&acc[j], &a_addr, b_addr, a_pitch, a_sbo, P.tap_off);
                 } else {
+                  uint32_t a_blk[GT];
 #pragma unroll
-                  for (int k = 0; k < GT; ++k) issue_stage<KG, TPG, NT>(acc[k], a_addr + boff[k], b_addr, a_pitch, a_sbo, P.tap_off);
+                  for (int k = 0; k < GT; ++k) a_blk[k] = a_addr + boff[k];
+                  issue_stage<KG, TPG, NT, GT>(acc, a_blk, b_addr, a_pitch, a_sbo, P.tap_off);
                 }
                 wg_commit();
                 wg_wait<1>();
@@ -645,21 +672,32 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   } else {
     P.tg_off[0] = 0; P.tap_off[0] = 0;
   }
+  const int n_tiles_n = w.cout_pad / NT;
   if (blk) {
     const int rp = P.rp, r = P.r;
     P.nzb = cdiv(r, 8); P.npl = P.nzb * P.nzb; P.nblk = r * P.npl;
-    // Blocks per group: two per accumulator set (one per warpgroup).  A group's window is its blocks' rows plus every
-    // tap's neighbours: from (y0-1, z0-1) of its first block to (y0+8, z0+8) of its last; the largest sets the stage.
-    // At N = 128 that is two whole x-planes at r = 8 (200 rows) and 8 y-lines x 16 z at r = 16 (180 rows).
-    const int ib = 2 * tc::tiles_per_item(NT);
-    int wrows = 0;
-    for (int f = 0; f < P.nblk; f += ib) {
-      const int l = std::min(f + ib, P.nblk) - 1;
-      wrows = std::max(wrows, tc::block_row(l, rp, P.nzb, P.npl) - tc::block_row(f, rp, P.nzb, P.npl) + 9 * rp + 10);
-    }
-    P.ib = ib;
-    P.stage_rows = wrows;
-    ntile = cdiv(P.nblk, ib);
+    // A group's window is its blocks' rows plus every tap's neighbours: from (y0-1, z0-1) of its first block to
+    // (y0+8, z0+8) of its last; the largest sets the stage.  At N = 128 that is two whole x-planes at r = 8 (200 rows)
+    // and 8 y-lines x 16 z at r = 16 (180 rows) for 2-block groups, one whole haloed x-plane (324 rows) for 4-block
+    // groups at r = 16.
+    auto window_rows = [&](int ib) {
+      int wrows = 0;
+      for (int f = 0; f < P.nblk; f += ib) {
+        const int l = std::min(f + ib, P.nblk) - 1;
+        wrows = std::max(wrows, tc::block_row(l, rp, P.nzb, P.npl) - tc::block_row(f, rp, P.nzb, P.npl) + 9 * rp + 10);
+      }
+      return wrows;
+    };
+    // Blocks per group: one per warpgroup, or two (two accumulator sets per thread), which doubles the MMAs of every
+    // weight slab and A stage and halves the per-slab barrier round trips, copy latencies and item epilogues.  4-block
+    // groups are taken while there are still as many groups as SMs, and while their window leaves one A stage more than
+    // the 2 weight slabs (each slab consumes one A stage).  At B = 32 that is r = 16 (512 groups, 3 A stages), not
+    // r = 8 (64 groups would idle half the SMs).
+    const long long a_room2 = 227LL * 1024 - (long long)fixed - 2LL * P.b_stage_bytes;
+    const bool four = (long long)n_tiles_n * B * cdiv(P.nblk, 4) >= c->num_sms && a_room2 / (KG * window_rows(4) * 16) >= 3;
+    P.ib = four ? 4 : 2;
+    P.stage_rows = window_rows(P.ib);
+    ntile = cdiv(P.nblk, P.ib);
     P.G = 1;
   } else {
     if (w.ntaps == 27) P.halo = P.rp + 1;
@@ -683,7 +721,6 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   }
   P.b_stages = b_stages;
   const long long a_room = 227LL * 1024 - (long long)fixed - (long long)b_stages * P.b_stage_bytes;
-  int n_tiles_n = w.cout_pad / NT;
   // Round-based items (sched 1) for 3x3x3 grids whose input is well beyond the L2: the three x-plane sweeps of a tile then
   // hit the L2 instead of re-reading DRAM.  Measured on an H100 SXM (400 W, B = 32, kernel alone, sched 0 / 1 alternated
   // twice): every grid above 1.6x the 50 MB L2 runs faster with rounds (64 ch @ 32^3, 322 MB: 7-9 %; 32 ch @ 32^3,
@@ -727,20 +764,22 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
     LION_LAUNCH(c, tc::k_conv_stats<128>, grid_for(ntile_rows), 256, 0, S);
     return check_launch(c, "conv_tc stats");
   };
-#define CONV_TC_CASE(kg, tpg_, nt_, blk_)                                                                 \
-  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_) {                                              \
+  const int bpw = blk ? P.ib / 2 : 1;
+  c->conv_group_blocks = blk ? P.ib : 0;
+#define CONV_TC_CASE(kg, tpg_, nt_, blk_, bpw_)                                                           \
+  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_ && bpw == bpw_) {                               \
     static DevOnce attr_once;                                                                             \
     if (attr_once.need()) {                                                                               \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
     }                                                                                                     \
-    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_>), grid, tc::THREADS, smem, P);                     \
+    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_>), grid, tc::conv_threads(bpw_), smem, P);    \
     LION_TRY(check_launch(c, "conv_tc"));                                                                 \
     return stats();                                                                                       \
   }
-#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false) CONV_TC_CASE(kg, tpg_, 64, false) CONV_TC_CASE(kg, tpg_, 96, false)
+#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false, 1) CONV_TC_CASE(kg, tpg_, 64, false, 1) CONV_TC_CASE(kg, tpg_, 96, false, 1)
   CONV_TC_NT(2, 1) CONV_TC_NT(4, 1) CONV_TC_NT(8, 1) CONV_TC_NT(2, 9) CONV_TC_NT(4, 9) CONV_TC_NT(8, 9)
-  CONV_TC_CASE(2, 1, 128, false) CONV_TC_CASE(4, 1, 128, false) CONV_TC_CASE(8, 1, 128, false)
-  CONV_TC_CASE(2, 9, 128, true) CONV_TC_CASE(4, 9, 128, true)
+  CONV_TC_CASE(2, 1, 128, false, 1) CONV_TC_CASE(4, 1, 128, false, 1) CONV_TC_CASE(8, 1, 128, false, 1)
+  CONV_TC_CASE(2, 9, 128, true, 1) CONV_TC_CASE(4, 9, 128, true, 1) CONV_TC_CASE(2, 9, 128, true, 2) CONV_TC_CASE(4, 9, 128, true, 2)
 #undef CONV_TC_NT
 #undef CONV_TC_CASE
   set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps", NT, KG, tpg);

@@ -37,9 +37,21 @@ static __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity
     if (clock64() - t0 > 2000000000LL) __trap();
   }
 }
-// warp-collective: lanes may leave the polling loop at different times, reconverge for the .aligned instructions after it
+// warp-collective: lanes may leave the polling loop at different times, reconverge for the .aligned instructions after it.
+// INLINE: the slow path without a call -- ptxas cannot allocate a kernel that changes its register count (setmaxnreg)
+// around a call.
+template <bool INLINE = false>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  if (!mbar_try(bar, parity)) mbar_wait_slow(bar, parity);
+  if (!mbar_try(bar, parity)) {
+    if constexpr (INLINE) {
+      const long long t0 = clock64();
+      while (!mbar_try(bar, parity)) {
+        if (clock64() - t0 > 2000000000LL) __trap();
+      }
+    } else {
+      mbar_wait_slow(bar, parity);
+    }
+  }
   __syncwarp();
 }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -55,6 +67,12 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t addr, uint32_t lbo_bytes,
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
   return d;
 }
+
+// hand registers of this warpgroup back to the CTA's pool / take them from it (every warp of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

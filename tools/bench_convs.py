@@ -50,13 +50,20 @@ def operand_bytes(ntaps, cin, cout, r_or_rows, B, num_sms, l2_bytes):
         kg = 2 if kg_all <= 2 else (4 if kg_all <= 4 else 8)
     nchunk, ntg, tpg = -(-kg_all // kg), (3 if ntaps == 27 else 1), (9 if ntaps == 27 else 1)
     b_stage = tpg * kg * nt * 16
-    if ntaps == 27 and nt == 128:                     # interior 8 x 8 blocks, groups of 2 per item
+    if ntaps == 27 and nt == 128:                     # interior 8 x 8 blocks, groups of 2 or 4 per item
         r, rp = r_or_rows, r_or_rows + 2
         nzb = -(-r // 8)
-        npl, ib = nzb * nzb, 2
+        npl = nzb * nzb
         nblk = r * npl
-        stage_rows = max(_block_row(min(f + ib, nblk) - 1, rp, nzb, npl) - _block_row(f, rp, nzb, npl) + 9 * rp + 10
-                         for f in range(0, nblk, ib))
+
+        def window(ib):
+            return max(_block_row(min(f + ib, nblk) - 1, rp, nzb, npl) - _block_row(f, rp, nzb, npl) + 9 * rp + 10
+                       for f in range(0, nblk, ib))
+        fixed = 128 * 4 + 8 * 2 * nt * 4 + 64 * 8 + 128 + 1024
+        four = (n_nt * B * -(-nblk // 4) >= num_sms
+                and (227 * 1024 - fixed - 2 * b_stage) // (kg * window(4) * 16) >= 3)
+        ib = 4 if four else 2
+        stage_rows = window(ib)
         ntile, G, rows = -(-nblk // ib), 1, rp ** 3
     else:                                             # 128-row tiles, up to G per item
         rp = r_or_rows + 2 if ntaps == 27 else 0
