@@ -149,6 +149,20 @@ int lion_swish_fwd(const float* x, float* out, size_t n, void* stream);
  * sum and the sum of squares of the outputs over the r^3 voxels.  TF32 operands, fp32 accumulation, like the
  * reference's cuDNN path under torch's default flags. */
 int lion_conv3d_gn_fwd(LionModel* m, const float* x, float* out, double* gn_sum, double* gn_sqsum, int B, void* stream);
+/* Stage probes for tests: the product code of one stage, with results a module's output hides.
+ * lion_pvconv_conv1_probe: a PVConv model's first convolution (voxelisation, scatter, convolution): out [B,Cout,r,r,r]
+ * raw output, gn_sum / gn_sqsum [B,Cout] its fused GroupNorm sums.  path: 0 = the path lion_pvconv_fwd chooses,
+ * 1 = dense tensor-core convolution, 2 = sparse; a forced path that cannot serve the layer is an error.  *path_taken
+ * (may be NULL) = 1 (dense) or 2 (sparse). */
+int lion_pvconv_conv1_probe(LionModel* m, const float* features, const float* coords, int path, float* out,
+                            double* gn_sum, double* gn_sqsum, int* path_taken, int B, int N, void* stream);
+/* lion_sa_mlp_probe: an SA model's MLP.  path: 0 = the path lion_sa_module_fwd chooses, 1 = unfused kernels, 2 = fused.
+ * Per layer l with C_l channels, at offset B * (C_0 + ... + C_{l-1}): gn_sum / gn_sqsum [B,C_l] (doubles) and the folded
+ * AdaGN scale / shift [B,C_l]; pool_mm [B][C_last/4][M][2][4] the minimum (index 0) and maximum (1) of the last layer's
+ * pre-activation over each centre's 32 neighbours; centers [B,3,M]; *path_taken (may be NULL) = 1 or 2. */
+int lion_sa_mlp_probe(LionModel* m, const float* features, const float* coords, const float* style, int path,
+                      float* centers, double* gn_sum, double* gn_sqsum, float* scale, float* shift, float* pool_mm,
+                      int* path_taken, int B, int N, void* stream);
 /* Prior.forward with SE cells (models/score_sde/resnet.py:195-218): x [B,D], t [B], clip [B,clip_dim] or NULL */
 int lion_global_prior_forward(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                               void* stream);

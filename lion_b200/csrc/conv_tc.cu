@@ -742,6 +742,11 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   if (a_stages > tc::MAX_A_STAGES) a_stages = tc::MAX_A_STAGES;
   if (a_stages < 2) { set_error("conv_tc: shared memory cannot hold the operand pipeline (N=%d, KG=%d)", NT, KG); return LION_ERR_ARG; }
   P.a_stages = a_stages;
+  // Occupancy skips need an A ring of two items' worth of row tiles.  A consumer hands the stage of its last MMA group
+  // back at its next issue; on a shallower ring a run of skipped stages comes round to that stage first, and producer and
+  // consumers wait for each other (4-tile items on the 6-stage ring of N = 32 with 32-channel chunks).  Without the flags
+  // the all-zero slabs are multiplied instead, which adds exact zeros.  (Block groups retire every slab.)
+  if (!blk && P.occ && a_stages < 2 * P.G) P.occ = nullptr;
   size_t smem = (size_t)a_stages * P.a_stage_bytes + (size_t)b_stages * P.b_stage_bytes + fixed;
   if (smem > 227 * 1024) { set_error("conv_tc: %zu bytes of shared memory needed", smem); return LION_ERR_ARG; }
   // persistent, at most one CTA per SM: the fewest CTAs that still reach the minimal maximum of tiles per CTA

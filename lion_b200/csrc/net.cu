@@ -242,13 +242,32 @@ int make_fp(Model* m, FPBlk& f, Cursor& cur, int cc, int cp, const std::vector<i
 struct PF { float4* p = nullptr; int G = 0; int R = 0; };
 struct VoxPrep { const float4* c4; int N, r; float4* nc; int* order; int* ppos; int* len; unsigned char* occ; int occ_stride;
                  int* cidx; int* nocc; int* vgrid; };   // compact ids of the occupied voxels (sparse first convolution) or null
+// Intermediate results of one SA module's MLP that lion_sa_mlp_probe copies out: device pointers into the forward's arena,
+// filled in by sa_fwd / shared_mlp_fwd when Fwd::rec is set (never in a product call).
+constexpr int MLP_REC_MAX = 4;
+struct MlpRecord {
+  int force = 0;                  // in: 0 = the path sa_fwd chooses, 1 = unfused kernels, 2 = fused (sa_fused.cu)
+  bool fused = false;             // out: the path that ran
+  int n = 0;                      // layers recorded
+  const double* ssum[MLP_REC_MAX]; const double* ssq[MLP_REC_MAX]; int stat_stride[MLP_REC_MAX];
+  const float* scale[MLP_REC_MAX]; const float* shift[MLP_REC_MAX];   // [B][C] folded AdaGN of each layer
+  const float* pool_mm = nullptr; // last layer: [B][C/4][M][2][4] pre-activation minimum / maximum over the 32 neighbours
+};
 struct Fwd {
   Ctx* c; Model* m; int B;
   char* stat_pool = nullptr;     // all GroupNorm statistics of a forward: zeroed by ONE memset
   size_t stat_off = 0, stat_cap = 0;
   float* aff = nullptr;          // [B][style_total] all AdaGN (factor|bias) vectors of this forward
   std::deque<VoxPrep> vox;       // a deque: get_vox hands out pointers that later preps must not move
+  MlpRecord* rec = nullptr;      // test entry points only
 };
+static void record_layer(Fwd& f, const AffSrc& a) {
+  MlpRecord* r = f.rec;
+  if (!r || r->n >= MLP_REC_MAX) return;
+  r->ssum[r->n] = a.ssum; r->ssq[r->n] = a.ssq; r->stat_stride[r->n] = a.stat_stride;
+  r->scale[r->n] = a.scale; r->shift[r->n] = a.shift;
+  r->n++;
+}
 // One point level of a forward: SA level i's input points, the centres its FPS samples from them (the points of
 // level i + 1) with their ball-query neighbours, and the 3-NN of the points among the centres that the FP stage
 // interpolating back onto them uses.  An event is set from the side stream's record of the result until the main
@@ -406,12 +425,15 @@ static int shared_mlp_fwd(Fwd& f, const SharedMLPBlk& m, PF in, int pool, float4
       LION_TRY(alloc_stats(f, w.cout_pad, &ssum, &ssq));
       LION_TRY(run_conv(f, w, cur.p, cur.G, nullptr, Gout, ssum, ssq, geom_rows(cur.R), mm));
       LION_TRY(run_affine(f, m.gn[i], ssum, ssq, w.cout_pad, (double)cur.R, nullptr, nullptr, a));
+      record_layer(f, a);
+      if (f.rec) f.rec->pool_mm = mm;
       LION_LAUNCH(f.c, k_act_pool_minmax, dim3(cdiv(Ro, 256), Gout, f.B), 256, 0, (const float4*)mm, dst, a, Gout, w.cout, Ro, Gd, g_off);
       LION_TRY(check_launch(f.c, "shared_mlp pooled"));
       continue;
     }
     PF raw = alloc_pf(f, Gout, cur.R);
     LION_TRY(conv_gn(f, w, cur.p, cur.G, raw.p, Gout, geom_rows(cur.R), m.gn[i], (double)cur.R, nullptr, nullptr, a));
+    record_layer(f, a);
     if (last && pool > 1) {
       if (pool != 32 || cur.R % 32) { set_error("shared_mlp: unsupported pooling %d", pool); return LION_ERR_ARG; }
       int Ro = cur.R / 32;
@@ -478,16 +500,23 @@ static int get_vox(Fwd& f, cudaStream_t s, const float4* c4, int N, int r, VoxPr
   return 0;
 }
 
-// PVConv: features PF [cin] + coords -> dst PF (cout) at (Gd, g_off)
-static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, float4* dst, int Gd, int g_off) {
-  int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
-  if (feat.G != Gin) { set_error("PVConv: got %d input channels, expected %d", feat.G * 4, p.cin); return LION_ERR_ARG; }
-  VoxPrep* vp;
-  LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
-  size_t mk = f.c->mark();
-  ConvGeom geo = geom_grid(r);
-  const bool sparse1 = vp->cidx && ygemm_usable(p.c1y) && feat.G == p.c1y.cin_pad / 4;
-  float4* g_in = nullptr;
+// The first convolution of a PVConv, scatter included: the raw output (a VG of cout channels) and its GroupNorm sums.
+// path: 0 = the product's choice (sparse when the grid is sparse enough and the wide packing serves it), 1 = the dense
+// tensor-core convolution with occupancy skip, 2 = sparse.  A dense run leaves the scattered voxels in the context's zero
+// grid (g_in): the caller restores it (k_act_grid's extra blocks).  after_scatter() runs between the scatter and the
+// convolution (pvconv_fwd launches its point branch there).
+struct Conv1Out { float4* raw = nullptr; double* ssum = nullptr; double* ssq = nullptr; float4* g_in = nullptr; bool sparse = false; };
+template <typename F>
+static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, int path, Conv1Out& o, F&& after_scatter) {
+  const int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
+  ConvGeom geo1 = geom_grid(r);
+  // (the tensor-core kernel still skips operand slabs whose 64-row occupancy flags are all clear)
+  geo1.occ = vp->occ; geo1.occ_stride = vp->occ_stride;
+  const bool sparse_ok = vp->cidx && ygemm_usable(p.c1y) && feat.G == p.c1y.cin_pad / 4;
+  if (path == 2 && !sparse_ok) { set_error("PVConv: the sparse first convolution cannot serve this layer / grid"); return LION_ERR_ARG; }
+  if (path == 1 && !conv_tc_usable(p.c1, geo1)) { set_error("PVConv: no tensor-core packing of the first convolution"); return LION_ERR_ARG; }
+  const bool sparse1 = path == 0 ? sparse_ok : path == 2;
+  o.sparse = sparse1;
   PF xc;
   if (sparse1) {
     // compact list of the occupied voxels' mean features (same values k_scatter would store into the grid)
@@ -497,21 +526,13 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
     // point -> voxel scatter-mean into the context's persistent all-zero grid (no per-call memset)
     size_t zbytes = sizeof(float4) * ((size_t)f.B * Gin * P + 2 * ((size_t)rp * rp + rp + 8));
     if (zbytes > f.c->zgrid_need) f.c->zgrid_need = zbytes;
-    g_in = f.c->dry ? (float4*)(uintptr_t)0x1000 : (float4*)f.c->zgrid + ((size_t)rp * rp + rp + 8);
-    LION_LAUNCH(f.c, k_scatter, dim3(cdiv(N, 128), Gin, f.B), 128, 0, feat.p, vp->order, vp->ppos, vp->len, g_in, Gin, N, P);
+    o.g_in = f.c->dry ? (float4*)(uintptr_t)0x1000 : (float4*)f.c->zgrid + ((size_t)rp * rp + rp + 8);
+    LION_LAUNCH(f.c, k_scatter, dim3(cdiv(N, 128), Gin, f.B), 128, 0, feat.p, vp->order, vp->ppos, vp->len, o.g_in, Gin, N, P);
   }
   stamp(f.c, f.c->stream, " scatter");
-  // point branch first: conv1x1 -> stats (its fold shares a launch with conv1's below; the activation is applied inside
-  // the devox kernel)
-  const ConvW& pw = p.point.conv[0];
-  PF rawp = alloc_pf(f, Gout, N);
-  AffSrc ap;
-  PrepJob jp, j1;
-  LION_TRY(conv_gn_deferred(f, pw, feat.p, feat.G, rawp.p, Gout, geom_rows(N), p.point.gn[0], (double)N, ap, jp));
-  // conv1 -> (stats) -> AdaGN + Swish
+  LION_TRY(after_scatter());
   float4* raw1 = alloc_vg(f, Gout, r);
-  AffSrc a1;
-  double V = (double)r * r * r;
+  o.raw = raw1;
   if (sparse1) {
     const int ld = 27 * p.c1.cout_pad;
     float* y = f.c->alloc_n<float>((size_t)f.B * N * ld);
@@ -537,13 +558,38 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
     else
       LION_LAUNCH(f.c, k_sparse_conv_gather<64>, grid, 32 * nwarp, smem, y, ld, vp->vgrid, p.c1.bias, raw1, s1, q1, p.c1.cout_pad, r, N);
     LION_TRY(check_launch(f.c, "sparse conv1"));
-    j1 = prep_job(f, p.g1, s1, q1, p.c1.cout_pad, V, nullptr, nullptr, a1);
+    o.ssum = s1; o.ssq = q1;
   } else {
-    // (the tensor-core kernel still skips operand slabs whose 64-row occupancy flags are all clear)
-    ConvGeom geo1 = geo;
-    geo1.occ = vp->occ; geo1.occ_stride = vp->occ_stride;
-    LION_TRY(conv_gn_deferred(f, p.c1, g_in, Gin, raw1, Gout, geo1, p.g1, V, a1, j1));
+    LION_TRY(alloc_stats(f, p.c1.cout_pad, &o.ssum, &o.ssq));
+    LION_TRY(run_conv(f, p.c1, o.g_in, Gin, raw1, Gout, o.ssum, o.ssq, geo1));
   }
+  return 0;
+}
+
+// PVConv: features PF [cin] + coords -> dst PF (cout) at (Gd, g_off)
+static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, float4* dst, int Gd, int g_off) {
+  int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
+  if (feat.G != Gin) { set_error("PVConv: got %d input channels, expected %d", feat.G * 4, p.cin); return LION_ERR_ARG; }
+  VoxPrep* vp;
+  LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
+  size_t mk = f.c->mark();
+  ConvGeom geo = geom_grid(r);
+  const ConvW& pw = p.point.conv[0];
+  PF rawp;
+  AffSrc ap;
+  PrepJob jp, j1;
+  // scatter -> point branch -> conv1 -> (stats) -> AdaGN + Swish.  The point branch is conv1x1 -> stats (its fold shares
+  // a launch with conv1's below; the activation is applied inside the devox kernel).
+  Conv1Out c1;
+  LION_TRY(pvconv_conv1(f, p, feat, vp, 0, c1, [&]() -> int {
+    rawp = alloc_pf(f, Gout, N);
+    return conv_gn_deferred(f, pw, feat.p, feat.G, rawp.p, Gout, geom_rows(N), p.point.gn[0], (double)N, ap, jp);
+  }));
+  const bool sparse1 = c1.sparse;
+  float4 *raw1 = c1.raw, *g_in = c1.g_in;
+  AffSrc a1;
+  const double V = (double)r * r * r;
+  j1 = prep_job(f, p.g1, c1.ssum, c1.ssq, p.c1.cout_pad, V, nullptr, nullptr, a1);
   LION_TRY(run_prep(f, j1, &jp));
   stamp(f.c, f.c->stream, " conv1");
   // AdaGN-1 + Swish as a stand-alone pass over the grid (HBM-bound).  Folding it into conv2's operand staging
@@ -648,7 +694,7 @@ static int sa_fwd(Fwd& f, const SABlk& s, PF feat, Level& lv, float4* dst, int G
   if (feat.G != Gf) { set_error("SA: got %d feature channels, expected %d", feat.G * 4, s.cfeat); return LION_ERR_ARG; }
   size_t mk = f.c->mark();
   LION_TRY(wait_once(f.c, lv.sa_done));
-  if (sa_fused_usable(s)) {
+  if (sa_fused_usable(s) && !(f.rec && f.rec->force == 1)) {
     // gather -> conv -> AdaGN/Swish -> conv -> max-pool in two fused passes (sa_fused.cu): no [B, C, M, 32] round trips
     const ConvW &c1 = s.mlp.conv[0], &c2 = s.mlp.conv[1];
     double *s1, *q1, *s2, *q2;
@@ -660,6 +706,7 @@ static int sa_fwd(Fwd& f, const SABlk& s, PF feat, Level& lv, float4* dst, int G
     float* mm = f.c->alloc_n<float>((size_t)f.B * (c2.cout / 4) * M * 8);
     LION_TRY(sa_fused_run(f.c, s, feat.p, lv.pts, lv.centers, lv.nidx, a1.scale, a1.shift, s2, q2, c2.cout_pad, mm, f.B, N));
     LION_TRY(run_affine(f, s.mlp.gn[1], s2, q2, c2.cout_pad, (double)M * U, nullptr, nullptr, a2));
+    if (f.rec) { record_layer(f, a1); record_layer(f, a2); f.rec->pool_mm = mm; f.rec->fused = true; }
     LION_LAUNCH(f.c, k_act_pool_minmax, dim3(cdiv(M, 256), c2.cout / 4, f.B), 256, 0, (const float4*)mm, dst, a2, c2.cout / 4, c2.cout, M,
                 Gd, g_off);
     LION_TRY(check_launch(f.c, "sa fused"));
@@ -1443,6 +1490,91 @@ extern "C" int lion_conv3d_gn_fwd(LionModel* h, const float* x, float* out, doub
                                         cudaMemcpyDeviceToDevice, f.c->stream));
     }
     return check_launch(f.c, "lion_conv3d_gn_fwd");
+  });
+}
+
+// ---- stage probes: intermediate results of the product code that a module's output hides (tests only) -------------
+// A PVConv's first convolution as pvconv_fwd runs it (voxel prep, scatter, dense or sparse convolution with its fused
+// GroupNorm sums).  path: 0 = pvconv_fwd's choice, 1 = dense, 2 = sparse; *path_taken = 1 or 2.
+extern "C" int lion_pvconv_conv1_probe(LionModel* h, const float* features, const float* coords, int path, float* out,
+                                       double* gn_sum, double* gn_sqsum, int* path_taken, int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_PVCONV, "lion_pvconv_conv1_probe: not a pvconv model");
+  LION_REQUIRE(features && coords && out && gn_sum && gn_sqsum && path >= 0 && path <= 2 && B > 0 && N > 0,
+               "lion_pvconv_conv1_probe: bad arguments");
+  Model* m = &h->m;
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    const PVConvBlk& p = m->block->pv;
+    const int r = p.r, rp = r + 2, P = rp * rp * rp, Gout = p.cout / 4;
+    PF x = to_pf(f, features, m->desc[0], N);
+    float4* c4 = to_c4(f, coords, N);
+    VoxPrep* vp;
+    LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
+    Conv1Out c1;
+    LION_TRY(pvconv_conv1(f, p, x, vp, path, c1, [] { return 0; }));
+    // the dense path scattered into the context's zero grid: zero those voxels again (k_act_grid's extra blocks alone)
+    if (!c1.sparse)
+      LION_LAUNCH(f.c, k_act_grid, dim3(cdiv(N, 256), Gout, B), 256, 0, c1.raw, nullptr, AffSrc{}, Gout, p.cout, rp, P, 0,
+                  vp->ppos, c1.g_in, p.cin / 4, N);
+    LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), Gout, B), 256, 0, c1.raw, out, p.cout, Gout, r);
+    if (!f.c->dry) {
+      LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sum, sizeof(double) * p.cout, c1.ssum, sizeof(double) * p.c1.cout_pad,
+                                        sizeof(double) * p.cout, B, cudaMemcpyDeviceToDevice, f.c->stream));
+      LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sqsum, sizeof(double) * p.cout, c1.ssq, sizeof(double) * p.c1.cout_pad,
+                                        sizeof(double) * p.cout, B, cudaMemcpyDeviceToDevice, f.c->stream));
+      if (path_taken) *path_taken = c1.sparse ? 2 : 1;
+    }
+    return check_launch(f.c, "lion_pvconv_conv1_probe");
+  });
+}
+
+// An SA module's MLP as sa_fwd runs it.  path: 0 = sa_fwd's choice, 1 = unfused kernels, 2 = fused; *path_taken = 1 or 2.
+// Per layer l (C_l channels, offsets o_l = B * (C_0 + ... + C_{l-1})): gn_sum / gn_sqsum [B][C_l] doubles and the folded
+// AdaGN scale / shift [B][C_l] at o_l; pool_mm [B][C_last/4][M][2][4] = per (centre, channel) minimum and maximum of the
+// last layer's pre-activation over the 32 neighbours; centers [B,3,M].
+extern "C" int lion_sa_mlp_probe(LionModel* h, const float* features, const float* coords, const float* style, int path,
+                                 float* centers, double* gn_sum, double* gn_sqsum, float* scale, float* shift, float* pool_mm,
+                                 int* path_taken, int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_SA, "lion_sa_mlp_probe: not an SA model");
+  LION_REQUIRE(features && coords && (style || h->m.desc[4] == 0) && centers && gn_sum && gn_sqsum && scale && shift && pool_mm &&
+               path >= 0 && path <= 2 && B > 0 && N > 0, "lion_sa_mlp_probe: bad arguments");
+  Model* m = &h->m;
+  const SABlk& s = m->block->sa;
+  LION_REQUIRE((int)s.mlp.conv.size() <= MLP_REC_MAX, "lion_sa_mlp_probe: more than %d layers", MLP_REC_MAX);
+  LION_REQUIRE(path != 2 || sa_fused_usable(s), "lion_sa_mlp_probe: the fused kernels do not serve this module");
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    MlpRecord rec;
+    rec.force = path;
+    f.rec = &rec;
+    LION_TRY(style_affine_all(f, style ? style : f.c->alloc_n<float>((size_t)B * 4)));
+    PF x = to_pf(f, features, s.cfeat, N);
+    Level lv{to_c4(f, coords, N), N};
+    lv.centers = f.c->alloc_n<float4>((size_t)B * s.m);
+    PF o = alloc_pf(f, s.mlp.cout() / 4, s.m);
+    LION_TRY(sa_geometry(f, f.c->stream, s, lv, 0));
+    LION_TRY(sa_fwd(f, s, x, lv, o.p, o.G, 0));
+    if (rec.n != (int)s.mlp.conv.size() || !rec.pool_mm) {
+      set_error("lion_sa_mlp_probe: the last layer does not run the pooled epilogue");
+      return LION_ERR_ARG;
+    }
+    if (!f.c->dry) {
+      // (the arena sa_fwd released is not reused before these copies: they are the next work on the stream)
+      size_t off = 0;
+      for (int l = 0; l < rec.n; ++l) {
+        const int C = s.mlp.conv[l].cout;
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sum + off, sizeof(double) * C, rec.ssum[l], sizeof(double) * rec.stat_stride[l],
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sqsum + off, sizeof(double) * C, rec.ssq[l], sizeof(double) * rec.stat_stride[l],
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpyAsync(scale + off, rec.scale[l], sizeof(float) * B * C, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpyAsync(shift + off, rec.shift[l], sizeof(float) * B * C, cudaMemcpyDeviceToDevice, f.c->stream));
+        off += (size_t)B * C;
+      }
+      LION_CHECK_CUDA(cudaMemcpyAsync(pool_mm, rec.pool_mm, sizeof(float) * B * s.mlp.cout() * s.m * 2, cudaMemcpyDeviceToDevice,
+                                      f.c->stream));
+      if (path_taken) *path_taken = rec.fused ? 2 : 1;
+    }
+    LION_LAUNCH(f.c, k_c4_to_cm, dim3(cdiv(s.m, 256), B), 256, 0, lv.centers, centers, s.m);
+    return check_launch(f.c, "lion_sa_mlp_probe");
   });
 }
 

@@ -261,7 +261,8 @@ k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict
   float cs[2][CPL], cq[2][CPL];
 #pragma unroll
   for (int k = 0; k < CPL; ++k) { cs[0][k] = cs[1][k] = 0.0f; cq[0][k] = cq[1][k] = 0.0f; }
-  const int nlive = max(0, min(32, V - (blockIdx.x * nw + wid) * 32));
+  // (signed: with the unsigned blockIdx.x the difference wraps for the warps past V, and min() then counts 32 rows)
+  const int nlive = max(0, min(32, V - ((int)blockIdx.x * nw + wid) * 32));
   for (int j = 0; j < nlive; j += 2) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {

@@ -1,0 +1,172 @@
+"""Float64 references of two tensor-core stages -- the first convolution of a PVConv (dense or sparse) and the SA
+module's MLP -- with their operands modelled the way the kernels hand them to the tensor cores, and the point clouds
+the stage tests run them on.
+
+Operand model (TF32 = 10 explicit mantissa bits):
+  * packed weights are rounded to nearest, ties away from zero (cvt.rna, csrc/conv_tc.cu), like every operand a kernel
+    rounds itself (k_act_rows with flag 1, the fused SA pass 2);
+  * an fp32 operand that no kernel rounds (the scatter grid, the compact voxel list, the gathered SA rows) is read by
+    the tensor core with its low 13 mantissa bits ignored: truncation toward zero.
+"""
+import numpy as np
+import torch
+
+from oracle import point_ops as OP
+
+
+def tf32_rna(x):
+    """cvt.rna.tf32.f32: round the magnitude to 10 mantissa bits, ties away from zero."""
+    i = x.contiguous().view(torch.int32)
+    return ((i + 0x1000) & ~0x1fff).view(torch.float32)
+
+
+def tf32_trunc(x):
+    """An fp32 operand as the tensor core reads it in TF32 mode: the low 13 mantissa bits dropped."""
+    i = x.contiguous().view(torch.int32)
+    return (i & ~0x1fff).view(torch.float32)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# point clouds [3, N]
+# ---------------------------------------------------------------------------------------------------------------------
+def gaussian_cloud(seed, N, scale=0.4):
+    g = torch.Generator().manual_seed(seed)
+    return torch.randn(3, N, generator=g) * scale
+
+
+def clustered_cloud(N):
+    """Every point but six at the origin, one voxel; the six on the axes at distance 1 land on the grid's faces
+    (voxel coordinate 0 or r - 1).  Occupancy 7 at every resolution; one voxel list of N - 6 points."""
+    c = torch.zeros(3, N)
+    for k, (a, s) in enumerate([(0, 1.0), (0, -1.0), (1, 1.0), (1, -1.0), (2, 1.0), (2, -1.0)]):
+        c[a, N - 6 + k] = s
+    return c
+
+
+def sites_cloud(K, N, r, seed):
+    """K well-separated sites, each repeated, occupying exactly K voxels at (even) resolution r.
+
+    In voxel units u, two anchors at (+-r/2, 0, 0) fix the largest centred norm at r/2, so a site u with |u| < r/2
+    lands on voxel u + r/2 exactly (normalisation: (c - mean) / (2 max |c - mean|) + 1/2, times r).  Sites come in
+    pairs +-u with equal repeat counts (plus the origin when K is odd), so the mean stays 0 and no site drifts."""
+    assert r % 2 == 0 and 2 <= K <= N
+    h = r // 2
+    rng = np.random.default_rng(seed)
+    ax = np.arange(-(h - 1), h)
+    u = np.stack(np.meshgrid(ax, ax, ax, indexing="ij"), -1).reshape(-1, 3)
+    pos = (u[:, 0] > 0) | ((u[:, 0] == 0) & ((u[:, 1] > 0) | ((u[:, 1] == 0) & (u[:, 2] > 0))))   # one of each +-u
+    u = u[pos & ((u * u).sum(1) < (h - 0.5) ** 2) & ~((u[:, 0] == h - 1) & (u[:, 1] == 0) & (u[:, 2] == 0))]
+    npairs = (K - 2) // 2
+    assert npairs <= len(u), (K, r)
+    pick = u[rng.permutation(len(u))[:npairs]]
+    sites = [np.array([h, 0, 0]), np.array([-h, 0, 0])]
+    for p in pick:
+        sites += [p, -p]
+    if K % 2:
+        sites.append(np.zeros(3, dtype=np.int64))
+    sites = np.stack(sites).astype(np.float64)
+    cnt = np.full(K, N // K)
+    left = N - cnt.sum()
+    i = 0
+    while left >= 2:                                   # extra points go to whole pairs
+        cnt[i] += 1; cnt[i + 1] += 1
+        left -= 2; i = (i + 2) % (K - K % 2)
+    if left:
+        cnt[K - 1] += 1                                # K odd: the origin
+    pts = np.repeat(sites, cnt, axis=0)[rng.permutation(N)]
+    return torch.from_numpy((pts * 0.03).T.astype(np.float32)).contiguous()
+
+
+def voxel_ids(coords, r):
+    """[B,3,N] -> the kernels' voxel index x r^2 + y r + z of every point (oracle, CUDA summation order)."""
+    _, vox = OP.voxel_coords_cuda_order(coords, r)
+    v = vox.to(torch.int64)
+    return v[:, 0] * r * r + v[:, 1] * r + v[:, 2]
+
+
+def occupancy(coords, r):
+    ids = voxel_ids(coords, r)
+    return [int(torch.unique(ids[b]).numel()) for b in range(ids.shape[0])]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# first convolution of a PVConv
+# ---------------------------------------------------------------------------------------------------------------------
+def scatter_grid(features, ids, r):
+    """The grid k_scatter / k_scatter_compact build: per voxel, its points in ascending order, acc = f0 * (1/n), then
+    acc = fma(f_k, 1/n, acc) (the compiler contracts the kernel's multiply-add).  features [B,C,N] fp32 on the device,
+    ids [B,N] -> [B,C,r,r,r] fp32."""
+    B, C, N = features.shape
+    dev = features.device
+    V = r ** 3
+    gid = (ids.to(dev) + torch.arange(B, device=dev)[:, None] * V).reshape(-1)          # [B*N] voxel of the batch
+    cnt = torch.zeros(B * V, dtype=torch.int64, device=dev).scatter_add_(0, gid, torch.ones_like(gid))
+    inv = (1.0 / cnt[gid].to(torch.float32)).double()
+    order = torch.argsort(gid * N + torch.arange(B * N, device=dev) % N)              # by voxel, then point
+    sg = gid[order]
+    first = torch.ones_like(sg, dtype=torch.bool)
+    first[1:] = sg[1:] != sg[:-1]
+    start = torch.cummax(torch.where(first, torch.arange(B * N, device=dev), torch.zeros_like(sg)), 0).values
+    rank = torch.empty_like(sg)
+    rank[order] = torch.arange(B * N, device=dev) - start
+    f = features.permute(0, 2, 1).reshape(B * N, C).double()
+    acc = torch.zeros(B * V, C, dtype=torch.float32, device=dev)
+    for k in range(int(rank.max()) + 1):
+        sel = rank == k
+        v = gid[sel]
+        t = f[sel] * inv[sel, None]
+        acc[v] = (t if k == 0 else acc[v].double() + t).float()
+    return acc.view(B, V, C).permute(0, 2, 1).reshape(B, C, r, r, r).contiguous()
+
+
+def conv3x3x3_f64(x, w, b):
+    """27 shifted float64 matmuls + bias: x [B,Ci,r,r,r], w [Co,Ci,3,3,3] -> [B,Co,r,r,r] (zero padding 1)."""
+    B, _, r = x.shape[0], x.shape[1], x.shape[2]
+    xp = torch.nn.functional.pad(x, (1, 1, 1, 1, 1, 1))
+    out = b.view(1, -1, 1, 1, 1).repeat(B, 1, r, r, r)
+    for kx in range(3):
+        for ky in range(3):
+            for kz in range(3):
+                out += torch.einsum("oc,bcxyz->boxyz", w[:, :, kx, ky, kz], xp[:, :, kx:kx + r, ky:ky + r, kz:kz + r])
+    return out
+
+
+def conv1_reference(features, coords, w, b, r):
+    """float64 reference of a PVConv's first convolution on the device of `features`."""
+    ids = voxel_ids(coords, r)
+    g = scatter_grid(features, ids, r)
+    return conv3x3x3_f64(tf32_trunc(g).double(), tf32_rna(w.to(features.device)).double(), b.to(features.device).double())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# SA MLP
+# ---------------------------------------------------------------------------------------------------------------------
+def sa_rows(features, coords, centers, nidx):
+    """Layer-1 operand [B, M, 32, 4 + Cf]: [p - c in fp32, 0 | features], as k_group_gather / the fused gather build it."""
+    B, Cf, N = features.shape
+    M, U = nidx.shape[1:]
+    idx = nidx.reshape(B, 1, M * U).long()
+    p = coords.gather(2, idx.expand(B, 3, M * U)).view(B, 3, M, U)
+    d = p - centers[:, :, :, None]
+    f = features.gather(2, idx.expand(B, Cf, M * U)).view(B, Cf, M, U)
+    z = torch.zeros(B, 1, M, U, dtype=features.dtype, device=features.device)
+    return torch.cat([d, z, f], 1).permute(0, 2, 3, 1).contiguous()
+
+
+def fold_affine(ssum, ssq, gamma, beta, fb, count):
+    """k_affine_prep in float64: GroupNorm(8) statistics from the per-channel sums, then AdaGN's factor / bias."""
+    B, C = ssum.shape
+    cpg = C // 8
+    n = count * cpg
+    mean = ssum.view(B, 8, cpg).sum(-1) / n
+    var = (ssq.view(B, 8, cpg).sum(-1) / n - mean * mean).clamp_min(0)
+    rstd = 1.0 / torch.sqrt(var + 1e-5)
+    mean, rstd = mean.repeat_interleave(cpg, 1), rstd.repeat_interleave(cpg, 1)
+    f, bb = fb[:, :C], fb[:, C:]
+    return rstd * gamma * f, (beta - mean * rstd * gamma) * f + bb
+
+
+def swish_act(v32, scale, shift):
+    """The next layer's operand: rna(swish(fma(v, scale, shift))), v fp32 [B,M,U,C], scale / shift fp32 [B,C]."""
+    a = (v32.double() * scale[:, None, None, :].double() + shift[:, None, None, :].double()).float().double()
+    return tf32_rna((a * torch.sigmoid(a)).float())
