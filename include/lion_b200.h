@@ -163,6 +163,20 @@ int lion_pvconv_conv1_probe(LionModel* m, const float* features, const float* co
 int lion_sa_mlp_probe(LionModel* m, const float* features, const float* coords, const float* style, int path,
                       float* centers, double* gn_sum, double* gn_sqsum, float* scale, float* shift, float* pool_mm,
                       int* path_taken, int B, int N, void* stream);
+/* lion_pvconv_probe: a whole PVConv as lion_pvconv_fwd runs it (C = cout).  raw1 / raw2 [B,C,r,r,r] the raw outputs of
+ * the two 3x3x3 convolutions; act1 [B,C,r+2,r+2,r+2] the AdaGN-1 + Swish grid the second convolution reads, halo
+ * included; rawp [B,C,N] the point branch's raw 1x1 output; sums [4][B][C] (doubles) the second convolution's GroupNorm
+ * sum and sum of squares, then the point branch's; affine [6][B][C] the folded scale and shift of AdaGN-1, of the point
+ * branch's AdaGN and of AdaGN-2 with the SE gate multiplied in; fused [B,C,N] devoxelised + point branch (the attention's
+ * input; without attention the module output); out [B,C,N] the module output; *conv2_kernel (may be NULL) = the second
+ * convolution's kernel: 0 SIMT, 1 tensor-core row tiles, 2 or 4 interior-block groups of that many blocks.  The grids of
+ * raw1, act1 and raw2 are NaN-filled before their producers run. */
+int lion_pvconv_probe(LionModel* m, const float* features, const float* coords, const float* style, float* raw1, float* act1,
+                      float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out, int* conv2_kernel,
+                      int B, int N, void* stream);
+/* lion_attention_probe: a linear attention as lion_linear_attention_fwd runs it.  qkv [B, 3*heads*32, N] (q, k, v of
+ * every head), o [B, heads*32, N] the output before the projection, out [B,C,N]. */
+int lion_attention_probe(LionModel* m, const float* x, float* qkv, float* o, float* out, int B, int N, void* stream);
 /* Prior.forward with SE cells (models/score_sde/resnet.py:195-218): x [B,D], t [B], clip [B,clip_dim] or NULL */
 int lion_global_prior_forward(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                               void* stream);

@@ -70,6 +70,8 @@ def _proto(lib):
         "lion_conv3d_gn_fwd": (P(vp, vp, vp, vp, vp, i, vp), i),
         "lion_pvconv_conv1_probe": (P(vp, vp, vp, i, vp, vp, vp, C.POINTER(i), i, i, vp), i),
         "lion_sa_mlp_probe": (P(vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
+        "lion_pvconv_probe": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
+        "lion_attention_probe": (P(vp, vp, vp, vp, vp, i, i, vp), i),
         "lion_global_prior_step": (P(vp, vp, vp, vp, vp, i, vp), i),
         "lion_workspace_bytes": (P(vp), sz),
         "lion_ddim_update": (P(vp, vp, vp, vp, vp, vp, sz, vp, vp), i),

@@ -253,6 +253,17 @@ struct MlpRecord {
   const float* scale[MLP_REC_MAX]; const float* shift[MLP_REC_MAX];   // [B][C] folded AdaGN of each layer
   const float* pool_mm = nullptr; // last layer: [B][C/4][M][2][4] pre-activation minimum / maximum over the 32 neighbours
 };
+// Intermediate results of one PVConv (and its attention) that lion_pvconv_probe / lion_attention_probe copy out: device
+// pointers into the forward's arena, filled in by pvconv_fwd / attn_fwd when Fwd::pv is set (never in a product call).
+// In that mode pvconv_fwd also fills its raw1, act1 and raw2 grids with NaNs (0xff bytes) before their producers run,
+// so that a read of a halo row nobody wrote shows up instead of depending on what the arena held.
+struct PvRecord {
+  const float4 *raw1 = nullptr, *act1 = nullptr, *raw2 = nullptr;   // VGs of cout channels (act1: halo included)
+  const float4 *rawp = nullptr, *fused = nullptr;                    // PFs: point-branch 1x1 output, devox + point branch
+  AffSrc a1{}, ap{}, a2{};        // AdaGN-1, point-branch AdaGN, AdaGN-2 with the SE gate: sums and folded scale / shift
+  int conv2 = -1;                 // 0 = SIMT, 1 = tensor-core row tiles, 2 / 4 = interior-block groups of that many blocks
+  const float4 *qkv = nullptr, *o = nullptr;                         // attention: PFs of 3 H 32 and H 32 channels
+};
 struct Fwd {
   Ctx* c; Model* m; int B;
   char* stat_pool = nullptr;     // all GroupNorm statistics of a forward: zeroed by ONE memset
@@ -260,6 +271,7 @@ struct Fwd {
   float* aff = nullptr;          // [B][style_total] all AdaGN (factor|bias) vectors of this forward
   std::deque<VoxPrep> vox;       // a deque: get_vox hands out pointers that later preps must not move
   MlpRecord* rec = nullptr;      // test entry points only
+  PvRecord* pv = nullptr;        // test entry points only
 };
 static void record_layer(Fwd& f, const AffSrc& a) {
   MlpRecord* r = f.rec;
@@ -292,6 +304,12 @@ static float4* alloc_vg(Fwd& f, int G, int r) {
   size_t P = (size_t)rp * rp * rp, guard = (size_t)rp * rp + rp + 8;
   float4* base = f.c->alloc_n<float4>((size_t)f.B * G * P + 2 * guard);
   return base + guard;
+}
+// probe mode (Fwd::pv): every float of the VG's B * G * (r+2)^3 rows becomes a NaN
+static int poison_vg(Fwd& f, float4* vg, int G, int r) {
+  if (!f.pv) return 0;
+  const size_t rp = r + 2;
+  return memset_async(f.c, vg, 0xff, sizeof(float4) * f.B * G * rp * rp * rp);
 }
 
 static int style_affine_all(Fwd& f, const float* style) {
@@ -462,6 +480,7 @@ static int attn_fwd(Fwd& f, const AttnBlk& a, PF x, float4* dst, int Gd, int g_o
   PF o = alloc_pf(f, hid / 4, N);
   LION_LAUNCH(f.c, k_attn_apply, dim3(cdiv(N, 128), a.heads, f.B), 128, 0, qkv.p, part, o.p, a.heads, N, S);
   LION_TRY(check_launch(f.c, "attention"));
+  if (f.pv) { f.pv->qkv = qkv.p; f.pv->o = o.p; }
   if (Gd != a.C / 4 || g_off != 0) { set_error("attention: destination must be a plain PF"); return LION_ERR_ARG; }
   return run_conv(f, a.out, o.p, o.G, dst, a.C / 4, nullptr, nullptr, geom_rows(N));
 }
@@ -533,6 +552,7 @@ static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, 
   LION_TRY(after_scatter());
   float4* raw1 = alloc_vg(f, Gout, r);
   o.raw = raw1;
+  LION_TRY(poison_vg(f, raw1, Gout, r));
   if (sparse1) {
     const int ld = 27 * p.c1.cout_pad;
     float* y = f.c->alloc_n<float>((size_t)f.B * N * ld);
@@ -596,6 +616,7 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   // ("transform on load") was parity-green but made the convolutions 3.5x slower (measured on the B200, before the
   // port to H100).  Its extra blocks re-zero the scatter grid (was: k_unscatter).
   float4* act1 = alloc_vg(f, Gout, r);
+  LION_TRY(poison_vg(f, act1, Gout, r));
   {
     const int nb_act = cdiv(P, 256 * ACT_U);
     LION_LAUNCH(f.c, k_act_grid, dim3(nb_act + (sparse1 ? 0 : cdiv(N, 256)), Gout, f.B), 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act,
@@ -604,15 +625,23 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   stamp(f.c, f.c->stream, " act1");
   // conv2 -> (stats) -> AdaGN + SE folded into one affine
   float4* raw2 = alloc_vg(f, Gout, r);
+  LION_TRY(poison_vg(f, raw2, Gout, r));
   AffSrc a2;
   LION_TRY(conv_gn(f, p.c2, act1, Gout, raw2, Gout, geo, p.g2, V, p.se1, p.se2, a2));
   stamp(f.c, f.c->stream, " conv2");
+  if (f.pv) {
+    PvRecord& R = *f.pv;
+    R.raw1 = raw1; R.act1 = act1; R.raw2 = raw2; R.rawp = rawp.p;
+    R.a1 = a1; R.ap = ap; R.a2 = a2;
+    R.conv2 = !conv_tc_usable(p.c2, geo) ? 0 : f.c->conv_group_blocks ? f.c->conv_group_blocks : 1;
+  }
   // voxel -> point gather (+ point branch)
   if (p.has_attn) {
     PF fused = alloc_pf(f, Gout, N);
     LION_LAUNCH(f.c, k_devox_fuse, dim3(cdiv(N, 128), Gout, f.B), 128, 0, raw2, vp->nc, a2.scale, a2.shift, rawp.p, ap,
                 fused.p, Gout, p.cout, N, r, P, Gout, 0);
     LION_TRY(check_launch(f.c, "pvconv"));
+    if (f.pv) f.pv->fused = fused.p;
     if (Gd != Gout || g_off != 0) {
       PF t = alloc_pf(f, Gout, N);
       LION_TRY(attn_fwd(f, p.attn, fused, t.p, Gout, 0));
@@ -623,6 +652,7 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   } else {
     LION_LAUNCH(f.c, k_devox_fuse, dim3(cdiv(N, 128), Gout, f.B), 128, 0, raw2, vp->nc, a2.scale, a2.shift, rawp.p, ap,
                 dst, Gout, p.cout, N, r, P, Gd, g_off);
+    if (f.pv) f.pv->fused = dst;    // (the probe's destination is a plain PF: Gd == Gout, g_off == 0)
   }
   LION_TRY(check_launch(f.c, "pvconv"));
   f.c->release(mk);   // grids are dead once the output PF is written (stream order keeps this safe)
@@ -1575,6 +1605,77 @@ extern "C" int lion_sa_mlp_probe(LionModel* h, const float* features, const floa
     }
     LION_LAUNCH(f.c, k_c4_to_cm, dim3(cdiv(s.m, 256), B), 256, 0, lv.centers, centers, s.m);
     return check_launch(f.c, "lion_sa_mlp_probe");
+  });
+}
+
+// A whole PVConv as lion_pvconv_fwd runs it, with the intermediate results of its second half (C = cout, V = r^3):
+// raw1 / raw2 [B,C,r,r,r] the two convolutions' raw outputs; act1 [B,C,r+2,r+2,r+2] the AdaGN-1 + Swish grid conv2
+// reads, halo included; rawp [B,C,N] the point branch's raw 1x1 output; sums [4][B][C] doubles: conv2's sum and sum of
+// squares, then the point branch's; affine [6][B][C]: scale / shift of AdaGN-1, of the point-branch AdaGN and of AdaGN-2
+// with the SE gate multiplied in; fused [B,C,N] devoxelised + point branch (the attention's input; without attention
+// the module output); out [B,C,N]; *conv2_kernel (may be NULL) = 0 SIMT, 1 row tiles, 2 / 4 interior-block groups.
+extern "C" int lion_pvconv_probe(LionModel* h, const float* features, const float* coords, const float* style, float* raw1,
+                                 float* act1, float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out,
+                                 int* conv2_kernel, int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_PVCONV, "lion_pvconv_probe: not a pvconv model");
+  LION_REQUIRE(features && coords && (style || h->m.desc[4] == 0) && raw1 && act1 && raw2 && rawp && sums && affine && fused &&
+               out && B > 0 && N > 0, "lion_pvconv_probe: bad arguments");
+  Model* m = &h->m;
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    const PVConvBlk& p = m->block->pv;
+    const int C = p.cout, G = C / 4, r = p.r, rp = r + 2;
+    PvRecord rec;
+    f.pv = &rec;
+    LION_TRY(style_affine_all(f, style ? style : f.c->alloc_n<float>((size_t)B * 4)));
+    PF x = to_pf(f, features, m->desc[0], N);
+    float4* c4 = to_c4(f, coords, N);
+    PF o = alloc_pf(f, G, N);
+    LION_TRY(pvconv_fwd(f, p, x, c4, o.p, o.G, 0));
+    // (the arena pvconv_fwd released is not reused before these copies: they are the next work on the stream)
+    LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), G, B), 256, 0, rec.raw1, raw1, C, G, r);
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(rp * rp * rp, 256), G, B), 256, 0, rec.act1, act1, C, G, rp * rp * rp);
+    LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), G, B), 256, 0, rec.raw2, raw2, C, G, r);
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.rawp, rawp, C, G, N);
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.fused, fused, C, G, N);
+    from_pf(f, o, out, C);
+    if (!f.c->dry) {
+      const size_t BC = (size_t)B * C;
+      const AffSrc* st[2] = {&rec.a2, &rec.ap};
+      for (int k = 0; k < 2; ++k) {
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(sums + (2 * k) * BC, sizeof(double) * C, st[k]->ssum, sizeof(double) * st[k]->stat_stride,
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(sums + (2 * k + 1) * BC, sizeof(double) * C, st[k]->ssq, sizeof(double) * st[k]->stat_stride,
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+      }
+      const AffSrc* af[3] = {&rec.a1, &rec.ap, &rec.a2};
+      for (int k = 0; k < 3; ++k) {
+        LION_CHECK_CUDA(cudaMemcpyAsync(affine + (2 * k) * BC, af[k]->scale, sizeof(float) * BC, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpyAsync(affine + (2 * k + 1) * BC, af[k]->shift, sizeof(float) * BC, cudaMemcpyDeviceToDevice, f.c->stream));
+      }
+      if (conv2_kernel) *conv2_kernel = rec.conv2;
+    }
+    return check_launch(f.c, "lion_pvconv_probe");
+  });
+}
+
+// A linear attention as lion_linear_attention_fwd runs it: qkv [B, 3 H 32, N] (q, k, v of every head), o [B, H 32, N]
+// the output before the projection, out [B,C,N].
+extern "C" int lion_attention_probe(LionModel* h, const float* x, float* qkv, float* o, float* out, int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_ATTN, "lion_attention_probe: not an attention model");
+  LION_REQUIRE(x && qkv && o && out && B > 0 && N > 0, "lion_attention_probe: bad arguments");
+  Model* m = &h->m;
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    const AttnBlk& a = *m->attn;
+    const int hid = a.heads * 32;
+    PvRecord rec;
+    f.pv = &rec;
+    PF xi = to_pf(f, x, a.C, N);
+    PF y = alloc_pf(f, a.C / 4, N);
+    LION_TRY(attn_fwd(f, a, xi, y.p, y.G, 0));
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), 3 * hid / 4, B), 256, 0, rec.qkv, qkv, 3 * hid, 3 * hid / 4, N);
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), hid / 4, B), 256, 0, rec.o, o, hid, hid / 4, N);
+    from_pf(f, y, out, a.C);
+    return check_launch(f.c, "lion_attention_probe");
   });
 }
 

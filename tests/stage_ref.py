@@ -1,6 +1,6 @@
-"""Float64 references of two tensor-core stages -- the first convolution of a PVConv (dense or sparse) and the SA
-module's MLP -- with their operands modelled the way the kernels hand them to the tensor cores, and the point clouds
-the stage tests run them on.
+"""Float64 references of the stages of a PVConv (first convolution, AdaGN-1 + Swish grid, second convolution, SE fold,
+point branch, devoxelisation), of the linear attention and of the SA module's MLP -- with their operands modelled the
+way the kernels hand them to the tensor cores -- and the point clouds the stage tests run them on.
 
 Operand model (TF32 = 10 explicit mantissa bits):
   * packed weights are rounded to nearest, ties away from zero (cvt.rna, csrc/conv_tc.cu), like every operand a kernel
@@ -131,11 +131,12 @@ def conv3x3x3_f64(x, w, b):
     return out
 
 
-def conv1_reference(features, coords, w, b, r):
+def conv1_reference(features, coords, w, b, r, tc=True):
     """float64 reference of a PVConv's first convolution on the device of `features`."""
+    rna, trunc = operand_models(tc)
     ids = voxel_ids(coords, r)
     g = scatter_grid(features, ids, r)
-    return conv3x3x3_f64(tf32_trunc(g).double(), tf32_rna(w.to(features.device)).double(), b.to(features.device).double())
+    return conv3x3x3_f64(trunc(g).double(), rna(w.to(features.device)).double(), b.to(features.device).double())
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -170,3 +171,103 @@ def swish_act(v32, scale, shift):
     """The next layer's operand: rna(swish(fma(v, scale, shift))), v fp32 [B,M,U,C], scale / shift fp32 [B,C]."""
     a = (v32.double() * scale[:, None, None, :].double() + shift[:, None, None, :].double()).float().double()
     return tf32_rna((a * torch.sigmoid(a)).float())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# second half of a PVConv: AdaGN-1 + Swish grid, second convolution, SE fold, point branch, devoxelisation
+#
+# `tc` selects the operand model: True for layers the tensor-core kernels run (output widths that are multiples of
+# 32), False for the SIMT kernels (and for comparisons with the fp32 oracle), which read every operand unrounded.
+# ---------------------------------------------------------------------------------------------------------------------
+def _ident(x):
+    return x
+
+
+def operand_models(tc):
+    """(weight model, model of an fp32 operand no kernel rounds) for a tensor-core (tc) or SIMT layer."""
+    return (tf32_rna, tf32_trunc) if tc else (_ident, _ident)
+
+
+def act_grid(raw1, scale, shift, rna=True):
+    """k_act_grid: rna(swish(fma(raw1, scale, shift))) on the interior, exactly 0 on the one-voxel halo.
+    raw1 fp32 [B,C,r,r,r], scale / shift fp32 [B,C] -> fp32 [B,C,r+2,r+2,r+2]."""
+    a = (raw1.double() * scale[:, :, None, None, None].double() + shift[:, :, None, None, None].double()).float().double()
+    y = (a * torch.sigmoid(a)).float()
+    if rna:
+        y = tf32_rna(y)
+    return torch.nn.functional.pad(y, (1, 1, 1, 1, 1, 1))
+
+
+def fold_se(ssum, ssq, gamma, beta, fb, count, w1, w2):
+    """k_affine_prep with the SE gate, in float64: fold AdaGN-2 from the sums, then SE3d's gate from the per-channel
+    mean of its output, mean(scale x + shift) = scale mean(x) + shift; the gate multiplies scale and shift."""
+    rs, rt = fold_affine(ssum, ssq, gamma, beta, fb, count)
+    m = rs * (ssum / count) + rt
+    gate = torch.sigmoid(torch.relu(m @ w1.double().T) @ w2.double().T)
+    return rs * gate, rt * gate
+
+
+def point_conv(features, w, b, tc=True):
+    """The point branch's raw 1x1 convolution in float64: features fp32 [B,Ci,N], w [Co,Ci,1] -> [B,Co,N]."""
+    rna, trunc = operand_models(tc)
+    w = rna(w.reshape(w.shape[0], -1).contiguous()).double()
+    return torch.einsum("oc,bcn->bon", w, trunc(features).double()) + b.double()[None, :, None]
+
+
+def trilinear_f64(grid, nc, r):
+    """Trilinear devoxelisation in float64: grid [B,C,r,r,r], nc [B,3,N] normalised coordinates in [0, r-1] ->
+    [B,C,N].  A corner whose weight is 0 (fractional part 0) is not read."""
+    B, C = grid.shape[:2]
+    f = grid.reshape(B, C, -1)
+    c = nc.to(grid.device).double()
+    lo = torch.floor(c)
+    d1 = c - lo
+    lo = lo.long()
+    hi = torch.minimum(lo + 1, torch.full_like(lo, r - 1))
+    out = 0
+    for kx in (0, 1):
+        for ky in (0, 1):
+            for kz in (0, 1):
+                ix, iy, iz = [(hi if k else lo)[:, a] for a, k in enumerate((kx, ky, kz))]
+                w = 1.0
+                for a, k in enumerate((kx, ky, kz)):
+                    w = w * (d1[:, a] if k else 1.0 - d1[:, a])
+                idx = (ix * r + iy) * r + iz
+                out = out + f.gather(2, idx[:, None, :].expand(B, C, idx.shape[-1])) * w[:, None, :]
+    return out
+
+
+def devox_fuse(raw2, s2, t2, nc, rawp, sp, tp):
+    """k_devox_fuse in float64: trilinear(raw2 * s2 + t2) at nc, plus swish(rawp * sp + tp).  raw2 [B,C,r,r,r],
+    rawp [B,C,N], scale / shift [B,C]."""
+    r = raw2.shape[-1]
+    g = raw2.double() * s2.double()[:, :, None, None, None] + t2.double()[:, :, None, None, None]
+    a = rawp.double() * sp.double()[:, :, None] + tp.double()[:, :, None]
+    return trilinear_f64(g, nc, r) + a * torch.sigmoid(a)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# linear attention
+# ---------------------------------------------------------------------------------------------------------------------
+def attn_qkv(x, wqkv, tc=True):
+    """to_qkv in float64: x fp32 [B,C,N], wqkv [3 H 32, C, 1, 1] -> [B, 3 H 32, N]."""
+    rna, trunc = operand_models(tc)
+    w = rna(wqkv.reshape(wqkv.shape[0], -1).contiguous()).double()
+    return torch.einsum("oc,bcn->bon", w, trunc(x).double())
+
+
+def attn_core(qkv, heads):
+    """k_attn_ctx + k_attn_apply in float64: softmax over the points of k, ctx = k v^T, o = ctx^T q.
+    qkv [B, 3 H 32, N] (channels ordered qkv, head, c) -> o [B, H 32, N]."""
+    B, _, N = qkv.shape
+    q, k, v = qkv.double().view(B, 3, heads, 32, N).unbind(1)
+    k = torch.softmax(k, dim=-1)
+    ctx = torch.einsum("bhdn,bhen->bhde", k, v)
+    return torch.einsum("bhde,bhdn->bhen", ctx, q).reshape(B, heads * 32, N)
+
+
+def attn_out(o, wo, bo, tc=True):
+    """to_out in float64: o fp32 [B, H 32, N], wo [C, H 32, 1, 1] -> [B,C,N]."""
+    rna, trunc = operand_models(tc)
+    w = rna(wo.reshape(wo.shape[0], -1).contiguous()).double()
+    return torch.einsum("oc,bcn->bon", w, trunc(o).double()) + bo.double()[None, :, None]

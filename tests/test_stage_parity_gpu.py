@@ -56,7 +56,8 @@ def _clouds(B, N, r, seed):
     """Gaussian, clustered and (at even r) 'sites' clouds with 127 / 128 / 129 / 256 occupied voxels -- k_ygemm's
     128-row block boundaries -- mixed in one batch, so that the occupancy differs from shape to shape."""
     if B >= 6:
-        kinds = ["gauss", "cluster"] + [("sites", k) for k in (127, 128, 129, 256) if k <= N and r % 2 == 0]
+        # (at most r^3 / 2 sites: the r = 8 grid holds the 127 - 129 sites clouds, not the 256 one)
+        kinds = ["gauss", "cluster"] + [("sites", k) for k in (127, 128, 129, 256) if k <= N and k < r ** 3 // 2 and r % 2 == 0]
     else:
         kinds = ["gauss", "cluster"] + ([("sites", 129 if N < 2048 else 256)] if r % 2 == 0 and N >= 256 else [])
     kinds = (kinds + ["gauss"] * B)[:B]
