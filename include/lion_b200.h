@@ -27,6 +27,12 @@ int lion_ctx_last_launches(LionCtx* ctx);
 /* voxel blocks per work item of the last 128-channel 3x3x3 convolution on this context: 2, or 4 when there are enough
  * groups to give every SM work (0 when the last convolution ran on 128-row tiles) */
 int lion_ctx_last_conv_group(LionCtx* ctx);
+/* taps per weight stage of the last tensor-core convolution on this context: 9 when each 3x3x3 weight slab (one channel
+ * chunk and x-plane) was streamed whole, 3 when it was streamed in three 3-tap parts, 1 for a 1x1 convolution */
+int lion_ctx_last_conv_stage_taps(LionCtx* ctx);
+/* For tests: on != 0 makes every later 3x3x3 convolution on this context stream whole weight slabs (the outputs are
+ * bitwise the same either way; only the shared-memory rings differ); 0 restores the automatic choice.  Returns 0. */
+int lion_ctx_set_conv_whole_slabs(LionCtx* ctx, int on);
 /* Scratch-arena generation: bumped whenever a call had to re-allocate the per-device arena or zero grid.  A CUDA graph
  * captured on this context has the arena addresses baked in; it must not be replayed once the generation changed
  * (lion_b200._lib.capture_graph checks this and raises). */

@@ -71,6 +71,10 @@ struct Ctx {
   int conv_smem_cap = 0;
   // blocks per group of the last tensor-core convolution on interior blocks (2 or 4; 0 when it ran on row tiles)
   int conv_group_blocks = 0;
+  // taps per weight stage of the last tensor-core convolution: 9 (whole 3x3x3 slabs), 3 (slabs in 3-tap parts) or 1 (1x1)
+  int conv_stage_taps = 0;
+  // set by tests only (lion_ctx_set_conv_whole_slabs): 3x3x3 weight slabs are always streamed whole
+  bool conv_whole_slabs = false;
   // LION_TIMELINE=1 (diagnostic, tools/timeline_step.py): %globaltimer stamps dropped into both streams at block
   // boundaries -- this image has no nsys, and a step's critical path across the two streams is not visible otherwise
   unsigned long long* d_stamps = nullptr;

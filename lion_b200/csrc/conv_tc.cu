@@ -23,7 +23,8 @@
 //     bytes viewed through a descriptor whose start address is shifted by (dy*(r+2)+dz) rows.  L2->SM traffic per
 //     MAC drops 9x versus reloading per tap.
 //   * B operand: weights pre-packed [n-tile][chunk][x-plane][tap][C/4][co][4] so one bulk copy
-//     brings the 9 taps of a (channel chunk, x-plane); a CTA reuses it for up to tiles_per_item row tiles or 2
+//     brings the 9 taps of a (channel chunk, x-plane) -- or, for interior blocks where that deepens the A ring, one of
+//     three copies of 3 taps each (Params::tps); a CTA reuses it for up to tiles_per_item row tiles or 2
 //     interior blocks per warpgroup, whose accumulators all stay in registers (<= 128 per thread).
 //   * Output contract: rows of [p_begin, p_end) are written (halo rows as zeros), except on interior blocks, which
 //     leave the halo rows as they were: every consumer of a 3x3x3 output reads interior rows only.  Each output's
@@ -56,7 +57,7 @@ constexpr int THREADS = 32 * CONSUMER_WARPS + 32;    // + warp 8, the producer
 __host__ __device__ constexpr int conv_threads(int BPW) { return BPW == 2 ? 32 * CONSUMER_WARPS + 128 : THREADS; }
 constexpr int PRODUCER_REGS = 96, CONSUMER_REGS = 200;
 constexpr int MAX_A_STAGES = 16;   // the A ring is as deep as shared memory allows (Params::a_stages)
-constexpr int MAX_B_STAGES = 4;   // the weight ring: 2 slabs, deeper for 3x3x3 where shared memory allows (Params::b_stages)
+constexpr int MAX_B_STAGES = 4;   // the weight ring: 2 slabs, deeper for 3x3x3 where shared memory allows, or 4 3-tap parts (Params::b_stages)
 constexpr int OCC_SMEM = 1024;       // bytes of per-item occupancy flags kept in shared memory (r <= 38)
 // row tiles per work item: their accumulators (NT / 2 registers per thread each, 64 in all) share one weight slab.  The
 // statistics pass (k_conv_stats) rebuilds the row tiles' GroupNorm grouping from it, so it must not change.  Interior
@@ -90,6 +91,7 @@ struct Params {
   int a_stage_bytes, b_stage_bytes, stage_rows;
   int a_stages;          // depth of the A ring
   int b_stages;          // depth of the weight ring
+  int tps;               // taps per weight stage: tpg (whole slabs), or 3 (3x3x3 slabs streamed in 3-tap parts)
   const unsigned char* occ;   // 64-row occupancy flags of the input (sparse first conv of a PVConv) or null
   int occ_stride;
   // pooled 1x1 (last layer of a set-abstraction MLP): instead of the [rows][C] result, write per 32 consecutive rows (the
@@ -106,10 +108,11 @@ __host__ __device__ __forceinline__ int block_row(int k, int rp, int nzb, int np
   return ((x + 1) * rp + 1 + 8 * yb) * rp + 1 + 8 * zb;
 }
 
-// all wgmmas of NB 64-row blocks (operands at a_addr[0 .. NB-1]) for one (channel chunk, tap group) of this warpgroup:
-// TPG taps x KG/2 k-steps, the blocks interleaved per k-step (each accumulator set d[k] still takes its taps and k-steps
-// in order; the blocks share the weight descriptors).  a_sbo is the distance between a block's 8-row groups: 128 B for
-// 64 consecutive rows, (r+2) * 16 B for 8 y-lines x 8 z.
+// all wgmmas of NB 64-row blocks (operands at a_addr[0 .. NB-1]) for TPG consecutive taps of one (channel chunk, tap
+// group) of this warpgroup (weights of the first at b_addr, row offsets tap_off[0 .. TPG-1]): TPG taps x KG/2 k-steps,
+// the blocks interleaved per k-step (each accumulator set d[k] still takes its taps and k-steps in order; the blocks
+// share the weight descriptors).  a_sbo is the distance between a block's 8-row groups: 128 B for 64 consecutive rows,
+// (r+2) * 16 B for 8 y-lines x 8 z.
 template <int KG, int TPG, int NT, int NB = 1>
 __device__ __forceinline__ void issue_stage(float (*d)[NT / 2], const uint32_t* a_addr, uint32_t b_addr, uint32_t a_pitch,
                                             uint32_t a_sbo, const int* tap_off) {
@@ -218,13 +221,14 @@ __device__ __forceinline__ void stat_flush(const Params& P, float* s_stat, int e
 }
 
 // BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), BPW of them per warpgroup and group (P.ib = 2 * BPW); otherwise
-// 128-row tiles
-template <int KG, int TPG, int NT, bool BLK, int BPW = 1>
+// 128-row tiles.  TPS: taps per weight stage (= P.tps), TPG or 3; a commit group's wgmmas are one static chain.
+template <int KG, int TPG, int NT, bool BLK, int BPW = 1, int TPS = TPG>
 __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
   constexpr int GT = BLK ? BPW : tiles_per_item(NT);   // accumulator sets per thread
   constexpr int NTHR = conv_threads(BPW);
   constexpr bool SETREG = NTHR > THREADS;              // registers moved from the producer warpgroup to the consumers
   constexpr int NACC = NT / 2;                  // accumulator registers per thread and tile
+  constexpr int NPARTS = TPG / TPS;             // weight stages per (channel chunk, x-plane) slab
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* sA = smem;
   const int A_STAGES = P.a_stages;
@@ -288,8 +292,17 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
     int nt, ntile;
     long long v0;
     int occ_shape = -1;                                // shape whose occupancy flags s_occ holds
+    const int slab_floats = P.tpg * KG * NT * 4;       // one (chunk, x-plane) of the packed weights: tpg taps
+    auto copy_weights = [&](const float* src) {        // the next weight stage: tps taps from src
+      mbar_wait<SETREG>(bar_empty_b + 8 * sb, pb ^ 1);
+      if (lane == 0) {
+        mbar_expect_tx(bar_full_b + 8 * sb, P.b_stage_bytes);
+        bulk_g2s(sB_addr + sb * (uint32_t)P.b_stage_bytes, src, P.b_stage_bytes, bar_full_b + 8 * sb);
+      }
+      if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
+    };
     while (items.next(nt, v0, ntile)) {
-      const float* wsrc = P.w + (size_t)nt * P.nchunk * P.ntg * (P.b_stage_bytes / 4);
+      const float* wsrc = P.w + (size_t)nt * P.nchunk * P.ntg * slab_floats;
       // lane l keeps (shape, row tile) of the item's tile l: one division per item, a shuffle per stage
       int my_b = 0, my_t = 0;
       if (lane < ntile) { const int vl = (int)v0 + lane; my_b = vl / ntile_total; my_t = vl - my_b * ntile_total; }
@@ -300,13 +313,10 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
           // the last sweep of an item is never skipped: every accumulator then receives at
           // least one (zero-initialising) MMA per item and needs no "was it touched" bookkeeping
           const bool may_skip = P.occ && !(cc == P.nchunk - 1 && tg == P.ntg - 1);
-          mbar_wait<SETREG>(bar_empty_b + 8 * sb, pb ^ 1);
-          if (lane == 0) {
-            mbar_expect_tx(bar_full_b + 8 * sb, P.b_stage_bytes);
-            bulk_g2s(sB_addr + sb * (uint32_t)P.b_stage_bytes, wsrc + (size_t)(cc * P.ntg + tg) * (P.b_stage_bytes / 4),
-                     P.b_stage_bytes, bar_full_b + 8 * sb);
-          }
-          if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
+          // the slab's first weight stage, its tiles' A stages, then the slab's other parts: the order in which the
+          // consumers wait for them
+          const float* slab = wsrc + (size_t)(cc * P.ntg + tg) * slab_floats;
+          copy_weights(slab);
           for (int j = 0; j < ntile; ++j) {
             const int bj = __shfl_sync(0xffffffffu, my_b, j), tj = __shfl_sync(0xffffffffu, my_t, j);
             // row tiles: the tile's 128 rows (3x3x3: plus rp+1 halo rows on each side, shifted to x-plane tg).  Interior
@@ -353,6 +363,7 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
               bulk_g2s(sA_addr + sa * (uint32_t)P.a_stage_bytes + lane * bytes, in_lane + row0, cnt * 16u, full);
             if (++sa == (uint32_t)A_STAGES) { sa = 0; pa ^= 1; }
           }
+          for (int s = 1; s < NPARTS; ++s) copy_weights(slab + (size_t)s * (P.b_stage_bytes / 4));
         }
       }
     }
@@ -399,48 +410,60 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
           boff[j] = (uint32_t)(block_row(k, P.rp, P.nzb, P.npl) - s_f + P.rp + 1) * 16u;
         }
       }
-      // A stage (and weight slab) handed back one commit group late (wait_group 1): the tensor cores work on the
-      // next stage while this warp checks that the previous one has been read
+      // A stage (and weight stage) handed back one commit group late (wait_group 1): the tensor cores work on the
+      // next group while this warp checks that the previous one has been read.  A slab streamed in parts is one
+      // commit group per (part, tile): every accumulator still takes taps 0-8 in order, and a tile's A stage is held
+      // until the group of its last part has completed.
       int pend_a = -1, pend_b = -1;
+      bool skip[BLK ? 1 : GT];
       for (int cc = 0; cc < P.nchunk; ++cc) {
         for (int tg = 0; tg < P.ntg; ++tg) {
-          mbar_wait<SETREG>(bar_full_b + 8 * sb, pb);
-          const uint32_t b_addr = b_ring + sb * (uint32_t)P.b_stage_bytes;
+          const uint32_t sa0 = sa, pa0 = pa;             // A stage of the slab's first tile
 #pragma unroll
-          for (int j = 0; j < (BLK ? 1 : GT); ++j) {
-            if (j < ntile) {
-              mbar_wait<SETREG>(bar_full_a + 8 * sa, pa);
-              const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
-              if (!s_skip[sa]) {
-                wg_fence();
-                if (!BLK) {
-                  issue_stage<KG, TPG, NT>(&acc[j], &a_addr, b_addr, a_pitch, a_sbo, P.tap_off);
-                } else {
-                  uint32_t a_blk[GT];
+          for (int s = 0; s < NPARTS; ++s) {
+            mbar_wait<SETREG>(bar_full_b + 8 * sb, pb);
+            const uint32_t b_addr = b_ring + sb * (uint32_t)P.b_stage_bytes;
+            const int* toff = P.tap_off + s * TPS;
+            bool issued = false;
+            sa = sa0; pa = pa0;
 #pragma unroll
-                  for (int k = 0; k < GT; ++k) a_blk[k] = a_addr + boff[k];
-                  issue_stage<KG, TPG, NT, GT>(acc, a_blk, b_addr, a_pitch, a_sbo, P.tap_off);
+            for (int j = 0; j < (BLK ? 1 : GT); ++j) {
+              if (j < ntile) {
+                if (s == 0) {
+                  mbar_wait<SETREG>(bar_full_a + 8 * sa, pa);
+                  skip[j] = s_skip[sa] != 0;
+                  if (skip[j]) { int st = (int)sa; release(st, bar_empty_a); }   // all-zero input slab: nothing to accumulate
                 }
-                wg_commit();
-                wg_wait<1>();
-                release(pend_a, bar_empty_a);
-                release(pend_b, bar_empty_b);
-                pend_a = (int)sa;
-              } else {
-                int s = (int)sa;                         // all-zero input slab: nothing to accumulate
-                release(s, bar_empty_a);
+                if (!skip[j]) {
+                  const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
+                  wg_fence();
+                  if (!BLK) {
+                    issue_stage<KG, TPS, NT>(&acc[j], &a_addr, b_addr, a_pitch, a_sbo, toff);
+                  } else {
+                    uint32_t a_blk[GT];
+#pragma unroll
+                    for (int k = 0; k < GT; ++k) a_blk[k] = a_addr + boff[k];
+                    issue_stage<KG, TPS, NT, GT>(acc, a_blk, b_addr, a_pitch, a_sbo, toff);
+                  }
+                  wg_commit();
+                  wg_wait<1>();
+                  release(pend_a, bar_empty_a);
+                  release(pend_b, bar_empty_b);
+                  if (s == NPARTS - 1) pend_a = (int)sa;  // the tile's last group: its A stage goes back after it
+                  issued = true;
+                }
+                if (++sa == (uint32_t)A_STAGES) { sa = 0; pa ^= 1; }
               }
-              if (++sa == (uint32_t)A_STAGES) { sa = 0; pa ^= 1; }
             }
+            if (pend_b >= 0) {                           // no group issued on this stage: retire the older one
+              wg_wait<0>();
+              release(pend_a, bar_empty_a);
+              release(pend_b, bar_empty_b);
+            }
+            if (issued) pend_b = (int)sb;                // the group in flight still reads this weight stage
+            else { int st = (int)sb; release(st, bar_empty_b); }
+            if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
           }
-          if (pend_b >= 0) {                             // no group issued on this slab: retire the older one
-            wg_wait<0>();
-            release(pend_a, bar_empty_a);
-            release(pend_b, bar_empty_b);
-          }
-          if (pend_a >= 0) pend_b = (int)sb;             // the group in flight still reads this weight slab
-          else { int s = (int)sb; release(s, bar_empty_b); }
-          if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
         }
       }
       wg_wait<0>();
@@ -652,7 +675,7 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   P.Gin = Gin; P.Gout_store = Gout_store; P.cout_pad = w.cout_pad;
   P.rows = geo.rows; P.p_begin = geo.p_begin; P.p_end = geo.p_end;
   P.ntg = w.tc.ntg; P.tpg = tpg; P.KG = KG; P.nchunk = w.tc.nchunk; P.NT = NT;
-  P.b_stage_bytes = tpg * KG * NT * 16;
+  const int slab_bytes = tpg * KG * NT * 16;     // the weights of one (channel chunk, x-plane)
   P.B = B;
   P.occ = geo.occ; P.occ_stride = geo.occ_stride;
   const size_t fixed = tc::smem_fixed(NT, tpg);
@@ -693,7 +716,7 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
     // groups are taken while there are still as many groups as SMs, and while their window leaves one A stage more than
     // the 2 weight slabs (each slab consumes one A stage).  At B = 32 that is r = 16 (512 groups, 3 A stages), not
     // r = 8 (64 groups would idle half the SMs).
-    const long long a_room2 = 227LL * 1024 - (long long)fixed - 2LL * P.b_stage_bytes;
+    const long long a_room2 = 227LL * 1024 - (long long)fixed - 2LL * slab_bytes;
     const bool four = (long long)n_tiles_n * B * cdiv(P.nblk, 4) >= c->num_sms && a_room2 / (KG * window_rows(4) * 16) >= 3;
     P.ib = four ? 4 : 2;
     P.stage_rows = window_rows(P.ib);
@@ -709,18 +732,6 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   }
   P.ntile = ntile;
   P.a_stage_bytes = KG * P.stage_rows * 16;
-  // The weight ring.  A block group takes one A stage per weight slab, so the copies run ahead of the tensor cores by
-  // as many slabs as the weight ring holds: deepen it to 3-4 while at least 4 A stages (and one per slab) still fit --
-  // under the side-stream cap when one is set.  Row tiles share a slab among up to 4 tiles and keep 2.
-  int b_stages = 2;
-  if (blk) {
-    const long long limit = (c->conv_smem_cap > 0 ? c->conv_smem_cap : 227LL * 1024) - (long long)fixed;
-    while (b_stages < tc::MAX_B_STAGES &&
-           (limit - (long long)(b_stages + 1) * P.b_stage_bytes) / P.a_stage_bytes >= std::max(4, b_stages + 1))
-      ++b_stages;
-  }
-  P.b_stages = b_stages;
-  const long long a_room = 227LL * 1024 - (long long)fixed - (long long)b_stages * P.b_stage_bytes;
   // Round-based items (sched 1) for 3x3x3 grids whose input is well beyond the L2: the three x-plane sweeps of a tile then
   // hit the L2 instead of re-reading DRAM.  Measured on an H100 SXM (400 W, B = 32, kernel alone, sched 0 / 1 alternated
   // twice): every grid above 1.6x the 50 MB L2 runs faster with rounds (64 ch @ 32^3, 322 MB: 7-9 %; 32 ch @ 32^3,
@@ -728,20 +739,60 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   // (one pair of runs of one 25 MB grid excepted), and one contiguous range per CTA is kept.
   const double in_bytes = (double)B * Gin * geo.rows * 16.0;
   P.sched = w.ntaps == 27 && in_bytes > 1.6 * c->l2_bytes ? 1 : 0;
-  int a_stages = (int)(a_room / P.a_stage_bytes);
-  // Sharing an SM with the side stream.  FPS and the neighbour searches run on the side stream during the first
-  // ~1 ms of a step (32 CTAs x <= 26 KB of shared memory, latency-bound); a persistent convolution CTA that claims all
-  // 227 KB cannot become resident on their SMs, and with the static item split the whole convolution then takes two
-  // waves (tools/timeline_step.py shows it).  While the caller
-  // flags side-stream work (Ctx::conv_smem_cap) the ring gives up a slot or two -- never below 4 -- and the side
-  // kernels opt into the maximum shared-memory carve-out, because an SM only hosts kernels of one carve-out at a time.
-  if (c->conv_smem_cap > 0 && a_stages >= 5) {
-    int capped = (int)(((long long)c->conv_smem_cap - (long long)fixed - (long long)b_stages * P.b_stage_bytes) / P.a_stage_bytes);
-    if (capped >= 4 && capped < a_stages) a_stages = capped;
+  // The rings for weight stages of tps taps each; returns the A ring's depth, 0 if it cannot hold 2 stages.
+  //   * Weight ring.  Whole slabs: 2.  A block group takes one A stage per weight slab, so the copies run ahead of the
+  //     tensor cores by as many slabs as the weight ring holds: deepen it to 3-4 while at least 4 A stages (and one per
+  //     slab) still fit -- under the side-stream cap when one is set.  Row tiles share a slab among up to 4 tiles and
+  //     keep 2.  3-tap parts: 4, the 3 parts of the slab in use and 1 in flight.
+  //   * A ring: what the weight ring and the fixed part leave of 227 KB (at most MAX_A_STAGES).  Sharing an SM with the
+  //     side stream: FPS and the neighbour searches run on the side stream during the first ~1 ms of a step (32 CTAs x
+  //     <= 26 KB of shared memory, latency-bound); a persistent convolution CTA that claims all 227 KB cannot become
+  //     resident on their SMs, and with the static item split the whole convolution then takes two waves
+  //     (tools/timeline_step.py shows it).  While the caller flags side-stream work (Ctx::conv_smem_cap) the ring gives
+  //     up a slot or two -- never below 4 -- and the side kernels opt into the maximum shared-memory carve-out, because
+  //     an SM only hosts kernels of one carve-out at a time.
+  auto ring = [&](int tps, int& b_stages) -> int {
+    const long long stage = (long long)slab_bytes / tpg * tps;
+    b_stages = tps == tpg ? 2 : tc::MAX_B_STAGES;
+    if (blk && tps == tpg) {
+      const long long limit = (c->conv_smem_cap > 0 ? c->conv_smem_cap : 227LL * 1024) - (long long)fixed;
+      while (b_stages < tc::MAX_B_STAGES && (limit - (b_stages + 1) * stage) / P.a_stage_bytes >= std::max(4, b_stages + 1))
+        ++b_stages;
+    }
+    int a_stages = (int)((227LL * 1024 - (long long)fixed - b_stages * stage) / P.a_stage_bytes);
+    if (c->conv_smem_cap > 0 && a_stages >= 5) {
+      const int capped = (int)(((long long)c->conv_smem_cap - (long long)fixed - b_stages * stage) / P.a_stage_bytes);
+      if (capped >= 4 && capped < a_stages) a_stages = capped;
+    }
+    a_stages = std::min(a_stages, tc::MAX_A_STAGES);
+    return a_stages >= 2 ? a_stages : 0;
+  };
+  // Weight stages: whole slabs (tpg taps), or -- block groups -- each slab streamed as 3 parts of 3 taps (taps 3s ..
+  // 3s+2 are one contiguous run of the packing), which shrinks the weight ring and leaves the A ring the room: at B = 32
+  // 5 A stages instead of 3 beside the weight ring at r = 16 (4-block groups) and 9 instead of 5 at r = 8.  Parts are
+  // taken when they deepen the A ring and it still holds G + 1 = 2 windows.  No deadlock: producer and consumers walk
+  // the same order (a slab's first part, its item's A stages, its other parts), and every release the producer waits
+  // for needs only stages copied before it -- a part goes back after the group that follows its last group, an A stage
+  // after the group that follows its last part's group, and a ring of >= G + 1 stages lets the producer copy that
+  // group's stage first.  Each output's products and their order are those of whole slabs (taps 0-8 of each chunk and
+  // x-plane, k-steps in order), so the choice changes no bit of any output.
+  //   Row tiles (N <= 64) keep whole slabs.  Their consumers wait on full A stages for 3.5 % of their time at r = 32
+  // and 6.6 % at r = 16 (clock64 around the waits, 64 -> 64, B = 32), and 3-tap parts -- a commit group of 12 instead
+  // of 36 wgmmas per tile, a barrier round trip per part -- measured 20-25 % slower there.  The 4-block groups at r = 16
+  // waited 9 % of their time on A stages and 16 % on weight slabs; see DESIGN 4.1 for the numbers.
+  int b_whole = 0, b_parts = 0;
+  const int a_whole = ring(tpg, b_whole);
+  const int a_parts = blk && !c->conv_whole_slabs ? ring(3, b_parts) : 0;
+  const bool parts = a_parts > a_whole && a_parts >= P.G + 1;
+  if (!parts && !a_whole) {
+    set_error("conv_tc: shared memory cannot hold the operand pipeline (N=%d, KG=%d)", NT, KG); return LION_ERR_ARG;
   }
-  if (a_stages > tc::MAX_A_STAGES) a_stages = tc::MAX_A_STAGES;
-  if (a_stages < 2) { set_error("conv_tc: shared memory cannot hold the operand pipeline (N=%d, KG=%d)", NT, KG); return LION_ERR_ARG; }
+  P.tps = parts ? 3 : tpg;
+  P.b_stage_bytes = slab_bytes / tpg * P.tps;
+  P.b_stages = parts ? b_parts : b_whole;
+  const int a_stages = parts ? a_parts : a_whole;
   P.a_stages = a_stages;
+  const int b_stages = P.b_stages;
   // Occupancy skips need an A ring of two items' worth of row tiles.  A consumer hands the stage of its last MMA group
   // back at its next issue; on a shallower ring a run of skipped stages comes round to that stage first, and producer and
   // consumers wait for each other (4-tile items on the 6-stage ring of N = 32 with 32-channel chunks).  Without the flags
@@ -771,23 +822,26 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   };
   const int bpw = blk ? P.ib / 2 : 1;
   c->conv_group_blocks = blk ? P.ib : 0;
-#define CONV_TC_CASE(kg, tpg_, nt_, blk_, bpw_)                                                           \
-  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_ && bpw == bpw_) {                               \
+  c->conv_stage_taps = P.tps;
+#define CONV_TC_CASE(kg, tpg_, nt_, blk_, bpw_, tps_)                                                     \
+  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_ && bpw == bpw_ && P.tps == tps_) {              \
     static DevOnce attr_once;                                                                             \
     if (attr_once.need()) {                                                                               \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
     }                                                                                                     \
-    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_>), grid, tc::conv_threads(bpw_), smem, P);    \
+    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_>), grid, tc::conv_threads(bpw_), smem, P); \
     LION_TRY(check_launch(c, "conv_tc"));                                                                 \
     return stats();                                                                                       \
   }
-#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false, 1) CONV_TC_CASE(kg, tpg_, 64, false, 1) CONV_TC_CASE(kg, tpg_, 96, false, 1)
+#define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false, 1, tpg_) CONV_TC_CASE(kg, tpg_, 64, false, 1, tpg_) CONV_TC_CASE(kg, tpg_, 96, false, 1, tpg_)
+#define CONV_TC_BLK(kg, bpw_) CONV_TC_CASE(kg, 9, 128, true, bpw_, 9) CONV_TC_CASE(kg, 9, 128, true, bpw_, 3)
   CONV_TC_NT(2, 1) CONV_TC_NT(4, 1) CONV_TC_NT(8, 1) CONV_TC_NT(2, 9) CONV_TC_NT(4, 9) CONV_TC_NT(8, 9)
-  CONV_TC_CASE(2, 1, 128, false, 1) CONV_TC_CASE(4, 1, 128, false, 1) CONV_TC_CASE(8, 1, 128, false, 1)
-  CONV_TC_CASE(2, 9, 128, true, 1) CONV_TC_CASE(4, 9, 128, true, 1) CONV_TC_CASE(2, 9, 128, true, 2) CONV_TC_CASE(4, 9, 128, true, 2)
+  CONV_TC_CASE(2, 1, 128, false, 1, 1) CONV_TC_CASE(4, 1, 128, false, 1, 1) CONV_TC_CASE(8, 1, 128, false, 1, 1)
+  CONV_TC_BLK(2, 1) CONV_TC_BLK(4, 1) CONV_TC_BLK(2, 2) CONV_TC_BLK(4, 2)
 #undef CONV_TC_NT
+#undef CONV_TC_BLK
 #undef CONV_TC_CASE
-  set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps", NT, KG, tpg);
+  set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps, %d per weight stage", NT, KG, tpg, P.tps);
   return LION_ERR_ARG;
 }
 

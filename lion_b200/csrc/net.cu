@@ -1204,6 +1204,12 @@ extern "C" int lion_ctx_destroy(LionCtx* h) {
 }
 extern "C" int lion_ctx_last_launches(LionCtx* h) { return h ? h->c.launches : 0; }
 extern "C" int lion_ctx_last_conv_group(LionCtx* h) { return h ? h->c.conv_group_blocks : 0; }
+extern "C" int lion_ctx_last_conv_stage_taps(LionCtx* h) { return h ? h->c.conv_stage_taps : 0; }
+extern "C" int lion_ctx_set_conv_whole_slabs(LionCtx* h, int on) {
+  LION_REQUIRE(h, "lion_ctx_set_conv_whole_slabs: null context");
+  h->c.conv_whole_slabs = on != 0;
+  return 0;
+}
 extern "C" unsigned lion_ctx_generation(LionCtx* h) { return h ? h->c.generation : 0; }
 extern "C" int lion_ctx_timeline(LionCtx* h, unsigned long long* t_ns, char* names, int max_entries) {
   LION_REQUIRE(h && t_ns && names && max_entries >= 0, "lion_ctx_timeline: null argument");

@@ -2,7 +2,9 @@
 python tools/bench_convs.py  -> table + JSON lines (CUDA events via lion_bench_conv).
 
 Next to each time: the operand bytes the launch moves from L2 into shared memory (operand_bytes) and the rate that
-makes -- the weight slabs every work item streams, and the activation windows of its tiles."""
+makes -- the weight slabs every work item streams, and the activation windows of its tiles -- and the shared-memory
+rings of the launch: taps per weight stage (9 = whole slabs, 3 = 3-tap parts, 1 = 1x1) and the depth of the
+activation ring.  WHOLE_SLABS=1 makes every 3x3x3 launch stream whole weight slabs (same outputs; for comparisons)."""
 import ctypes as C
 import json
 import os
@@ -92,7 +94,38 @@ def operand_bytes(ntaps, cin, cout, r_or_rows, B, num_sms, l2_bytes):
     return items, items * slabs * b_stage, U * slabs * kg * stage_rows * 16
 
 
+def a_ring(ntaps, cin, cout, r_or_rows, B, num_sms, tps):
+    """depth of the activation ring beside weight stages of tps taps (conv_tc_run's ring(), no side-stream cap)"""
+    nt = cout if cout < 128 else 128
+    kg_all = cin // 4
+    kg = 4 if (ntaps == 27 and nt > 64) else 8
+    if kg_all < kg:
+        kg = 2 if kg_all <= 2 else (4 if kg_all <= 4 else 8)
+    tpg = 9 if ntaps == 27 else 1
+    fixed = 128 * 4 + 8 * 2 * nt * 4 + (8 * 2 * nt * 4 if tpg == 1 else 0) + 64 * 8 + 128 + 1024
+    stage_b = tps * kg * nt * 16
+    if ntaps == 27 and nt == 128:
+        r, rp = r_or_rows, r_or_rows + 2
+        nzb = -(-r // 8)
+        nblk = r * nzb * nzb
+        slab = 9 * kg * nt * 16
+
+        def window(ib):
+            return max(_block_row(min(f + ib, nblk) - 1, rp, nzb, nzb * nzb) - _block_row(f, rp, nzb, nzb * nzb) + 9 * rp + 10
+                       for f in range(0, nblk, ib))
+        four = (cout // nt) * B * -(-nblk // 4) >= num_sms and (227 * 1024 - fixed - 2 * slab) // (kg * window(4) * 16) >= 3
+        stage_a = kg * window(4 if four else 2) * 16
+    else:
+        stage_a = kg * (128 + (2 * (r_or_rows + 3) if ntaps == 27 else 0)) * 16
+    b_stages = 2 if tps == tpg else 4
+    if ntaps == 27 and nt == 128 and tps == tpg:
+        while b_stages < 4 and (227 * 1024 - fixed - (b_stages + 1) * stage_b) // stage_a >= max(4, b_stages + 1):
+            b_stages += 1
+    return min(16, (227 * 1024 - fixed - b_stages * stage_b) // stage_a)
+
+
 torch.cuda.init()
+L.check(L.lib().lion_ctx_set_conv_whole_slabs(L.ctx(), 1 if os.environ.get("WHOLE_SLABS") == "1" else 0), "whole slabs")
 ITERS = int(os.environ.get("ITERS", "10"))      # ITERS=3000 CLOCKS=1: long enough for nvidia-smi to see the clock under load
 
 
@@ -121,10 +154,12 @@ for nt, ci, co, r, n, label in SHAPES:
     tf = fl.value / (ms.value * 1e-3) / 1e12
     tot += ms.value * n
     items, wb, ab = operand_bytes(nt, ci, co, r, B, props.multi_processor_count, props.L2_cache_size)
+    tps = L.lib().lion_ctx_last_conv_stage_taps(L.ctx())
     rec = {"shape": label, "ntaps": nt, "cin": ci, "cout": co, "r_or_rows": r, "B": B, "ms": round(ms.value, 4),
            "tflops_algorithmic": round(tf, 1), "launches_per_step": n, "items": items, "weight_gb": round(wb / 1e9, 3),
            "activation_gb": round(ab / 1e9, 3), "weight_share": round(wb / (wb + ab), 2),
-           "l2_to_smem_gbs": round((wb + ab) / (ms.value * 1e-3) / 1e9)}
+           "l2_to_smem_gbs": round((wb + ab) / (ms.value * 1e-3) / 1e9), "taps_per_weight_stage": tps,
+           "a_stages": a_ring(nt, ci, co, r, B, props.multi_processor_count, tps)}
     if th is not None:
         stop.set()
         th.join(timeout=2)
