@@ -117,6 +117,14 @@ int lion_model_refresh(LionModel* m);
  * out [B,N,num_classes] point-major. */
 int lion_unet_forward(LionModel* m, const float* x, const float* t, const float* style, const float* clip, float* out,
                       int B, int N, void* stream);
+/* Forward flags, chosen per call (a captured graph replays the mode it was captured in):
+ * LION_FWD_CONV_FP16 -- the autocast(float16) route: the second 3x3x3 convolution of every PVConv takes FP16 operands
+ * (activations and weights rounded to nearest even) and accumulates in fp32; its input grid is stored in FP16.
+ * Everything else, and every output, stays fp32.  The model's first FP16 call packs the FP16 weights (outside stream
+ * capture). */
+#define LION_FWD_CONV_FP16 1
+int lion_unet_forward_flags(LionModel* m, const float* x, const float* t, const float* style, const float* clip, float* out,
+                            int B, int N, int flags, void* stream);
 /* Hoist of the step-invariant part of PVCNN2Unet.forward out of the sampling loop: the CLIP mixing
  * (models/latent_points_ada.py:132-137) and the 61 AdaGN style Linears (models/adagn.py:59-61) are evaluated once for
  * style [B,S] (+ clip [B,clip_dim] or NULL) into a buffer owned by the model; lion_unet_forward calls with style == NULL
@@ -155,6 +163,10 @@ int lion_swish_fwd(const float* x, float* out, size_t n, void* stream);
  * sum and the sum of squares of the outputs over the r^3 voxels.  TF32 operands, fp32 accumulation, like the
  * reference's cuDNN path under torch's default flags. */
 int lion_conv3d_gn_fwd(LionModel* m, const float* x, float* out, double* gn_sum, double* gn_sqsum, int B, void* stream);
+/* flags LION_FWD_CONV_FP16: FP16 operands (x and the weights rounded to nearest even), fp32 accumulation, for the shapes
+ * the FP16 kernel serves (Cin = Cout in {32, 64, 128}); any other shape runs exactly as with flags = 0. */
+int lion_conv3d_gn_fwd_flags(LionModel* m, const float* x, float* out, double* gn_sum, double* gn_sqsum, int B, int flags,
+                             void* stream);
 /* Stage probes for tests: the product code of one stage, with results a module's output hides.
  * lion_pvconv_conv1_probe: a PVConv model's first convolution (voxelisation, scatter, convolution): out [B,Cout,r,r,r]
  * raw output, gn_sum / gn_sqsum [B,Cout] its fused GroupNorm sums.  path: 0 = the path lion_pvconv_fwd chooses,
@@ -180,6 +192,10 @@ int lion_sa_mlp_probe(LionModel* m, const float* features, const float* coords, 
 int lion_pvconv_probe(LionModel* m, const float* features, const float* coords, const float* style, float* raw1, float* act1,
                       float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out, int* conv2_kernel,
                       int B, int N, void* stream);
+/* the same with forward flags; under LION_FWD_CONV_FP16 act1 is the FP16 grid, widened to fp32 in the same layout */
+int lion_pvconv_probe_flags(LionModel* m, const float* features, const float* coords, const float* style, float* raw1,
+                            float* act1, float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out,
+                            int* conv2_kernel, int B, int N, int flags, void* stream);
 /* lion_attention_probe: a linear attention as lion_linear_attention_fwd runs it.  qkv [B, 3*heads*32, N] (q, k, v of
  * every head), o [B, heads*32, N] the output before the projection, out [B,C,N]. */
 int lion_attention_probe(LionModel* m, const float* x, float* qkv, float* o, float* out, int B, int N, void* stream);

@@ -54,6 +54,7 @@ def _proto(lib):
         "lion_model_destroy": (P(vp), i),
         "lion_model_refresh": (P(vp), i),
         "lion_unet_forward": (P(vp, vp, vp, vp, vp, vp, i, i, vp), i),
+        "lion_unet_forward_flags": (P(vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_unet_cache_style": (P(vp, vp, vp, i, vp), i),
         "lion_style_encoder_forward": (P(vp, vp, vp, i, i, vp), i),
         "lion_pvconv_fwd": (P(vp, vp, vp, vp, vp, i, i, vp), i),
@@ -70,9 +71,11 @@ def _proto(lib):
         "lion_ddpm_next_step": (P(vp, vp, i, vp), i),
         "lion_ddpm_fetch_noise": (P(vp, vp, vp, sz, vp), i),
         "lion_conv3d_gn_fwd": (P(vp, vp, vp, vp, vp, i, vp), i),
+        "lion_conv3d_gn_fwd_flags": (P(vp, vp, vp, vp, vp, i, i, vp), i),
         "lion_pvconv_conv1_probe": (P(vp, vp, vp, i, vp, vp, vp, C.POINTER(i), i, i, vp), i),
         "lion_sa_mlp_probe": (P(vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
         "lion_pvconv_probe": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
+        "lion_pvconv_probe_flags": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, i, vp), i),
         "lion_attention_probe": (P(vp, vp, vp, vp, vp, i, i, vp), i),
         "lion_global_prior_step": (P(vp, vp, vp, vp, vp, i, vp), i),
         "lion_workspace_bytes": (P(vp), sz),
@@ -135,6 +138,17 @@ def ptr(t):
 
 def stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+FWD_CONV_FP16 = 1     # LION_FWD_CONV_FP16 (include/lion_b200.h)
+
+
+def forward_flags():
+    """The forward flags of the current autocast state: FWD_CONV_FP16 inside torch.autocast("cuda", dtype=torch.float16)
+    (what the reference's `autocast(enable_autocast)` enables), 0 otherwise.  Outputs stay fp32 either way."""
+    if torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.float16:
+        return FWD_CONV_FP16
+    return 0
 
 
 _ctxs = {}

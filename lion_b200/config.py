@@ -53,7 +53,7 @@ _DEFAULT = {
             "embedding_type": "positional", "num_channels_dae": 2048, "num_cell_per_scale_dae": 8,
             "num_scales_dae": 2, "dropout": 0.2, "learn_mixing_logit": 1, "ode_sample": 0, "sde_type": "vpsde", "sigma2_0": 0.0,
             "sigma2_min": 1e-4, "sigma2_max": 0.99, "beta_start": 0.1, "beta_end": 20.0, "time_eps": 0.01, "ode_eps": 1e-5,
-            "train_ode_solver_tol": 1e-5,
+            "train_ode_solver_tol": 1e-5, "autocast_train": False,
             "prior_model": "models.latent_points_ada_localprior.PVCNN2Prior"},
     "clipforge": {"enable": 0, "feat_dim": 512},
     "data": {"tr_max_sample_points": 2048, "cond_on_cat": 0, "batch_size_test": 10},

@@ -36,7 +36,13 @@
 //     sum-of-squares per warp in shared memory, one fp64 atomic per channel per shape and item),
 //     warp 8 = bulk-copy producer.  4-block groups run 384 threads: warps 8-11 give registers to the consumers (see
 //     conv_threads) and warp 8 alone copies.
+//   * operand type OP: float (TF32 wgmma, 4 channels per 16-byte group, m64nNk8) or __half (FP16 wgmma, 8 channels per
+//     group, m64nNk16; the second 3x3x3 convolution of a PVConv under autocast).  A group is 16 bytes either way and one
+//     k-step consumes two of them through the same descriptors, so the tiling record, the rings, the copies and the
+//     epilogue are the same bytes; only the MMA instruction reads OP.
 #include <algorithm>
+#include <type_traits>
+#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "model.cuh"
@@ -113,7 +119,7 @@ __host__ __device__ __forceinline__ int block_row(int k, int rp, int nzb, int np
 // the blocks interleaved per k-step (each accumulator set d[k] still takes its taps and k-steps in order; the blocks
 // share the weight descriptors).  a_sbo is the distance between a block's 8-row groups: 128 B for 64 consecutive rows,
 // (r+2) * 16 B for 8 y-lines x 8 z.
-template <int KG, int TPG, int NT, int NB = 1>
+template <int KG, int TPG, int NT, int NB = 1, typename OP = float>
 __device__ __forceinline__ void issue_stage(float (*d)[NT / 2], const uint32_t* a_addr, uint32_t b_addr, uint32_t a_pitch,
                                             uint32_t a_sbo, const int* tap_off) {
   const uint64_t b0 = make_desc(b_addr, NT * 16, 128);
@@ -126,8 +132,11 @@ __device__ __forceinline__ void issue_stage(float (*d)[NT / 2], const uint32_t* 
 #pragma unroll
     for (int ks = 0; ks < KG / 2; ++ks)
 #pragma unroll
-      for (int k = 0; k < NB; ++k)
-        wgmma_tf32<NT>(d[k], a0[k] + toff + (uint64_t)((ks * 2 * a_pitch) >> 4), b0 + (uint64_t)(((t * KG + ks * 2) * NT * 16) >> 4), 1);
+      for (int k = 0; k < NB; ++k) {
+        const uint64_t a = a0[k] + toff + (uint64_t)((ks * 2 * a_pitch) >> 4), b = b0 + (uint64_t)(((t * KG + ks * 2) * NT * 16) >> 4);
+        if constexpr (std::is_same<OP, __half>::value) wgmma_f16<NT>(d[k], a, b, 1);
+        else wgmma_tf32<NT>(d[k], a, b, 1);
+      }
   }
 }
 
@@ -222,7 +231,8 @@ __device__ __forceinline__ void stat_flush(const Params& P, float* s_stat, int e
 
 // BLK: 3x3x3 on interior 8 x 8 blocks (TPG == 9), BPW of them per warpgroup and group (P.ib = 2 * BPW); otherwise
 // 128-row tiles.  TPS: taps per weight stage (= P.tps), TPG or 3; a commit group's wgmmas are one static chain.
-template <int KG, int TPG, int NT, bool BLK, int BPW = 1, int TPS = TPG>
+// OP: operand type of the MMAs (float = TF32, __half = FP16), see the header.
+template <int KG, int TPG, int NT, bool BLK, int BPW = 1, int TPS = TPG, typename OP = float>
 __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
   constexpr int GT = BLK ? BPW : tiles_per_item(NT);   // accumulator sets per thread
   constexpr int NTHR = conv_threads(BPW);
@@ -438,12 +448,12 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
                   const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
                   wg_fence();
                   if (!BLK) {
-                    issue_stage<KG, TPS, NT>(&acc[j], &a_addr, b_addr, a_pitch, a_sbo, toff);
+                    issue_stage<KG, TPS, NT, 1, OP>(&acc[j], &a_addr, b_addr, a_pitch, a_sbo, toff);
                   } else {
                     uint32_t a_blk[GT];
 #pragma unroll
                     for (int k = 0; k < GT; ++k) a_blk[k] = a_addr + boff[k];
-                    issue_stage<KG, TPS, NT, GT>(acc, a_blk, b_addr, a_pitch, a_sbo, toff);
+                    issue_stage<KG, TPS, NT, GT, OP>(acc, a_blk, b_addr, a_pitch, a_sbo, toff);
                   }
                   wg_commit();
                   wg_wait<1>();
@@ -626,8 +636,36 @@ __global__ void k_pack_tc(const float* __restrict__ wt, float* __restrict__ w, i
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(v));
   w[i] = __uint_as_float(u);
 }
+// the FP16 packing of the same weights for the FP16 kernels: w16[nt][chunk][tg][t][kg][n][8], rounded to nearest even
+// (what tensor.half() does); a 16-byte group holds 8 input channels
+__global__ void k_pack_tc16(const float* __restrict__ wt, __half* __restrict__ w, int ntaps, int cin_pad, int cout_pad,
+                            int NT, int nchunk, int ntg, int tpg, int KG) {
+  size_t total = (size_t)(cout_pad / NT) * nchunk * ntg * tpg * KG * NT * 8;
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  int jj = i % 8;
+  size_t r = i / 8;
+  int n = r % NT; r /= NT;
+  int kg = r % KG; r /= KG;
+  int t = r % tpg; r /= tpg;
+  int tg = r % ntg; r /= ntg;
+  int cc = r % nchunk; r /= nchunk;
+  int nt = (int)r;
+  int tap = tg * tpg + t;
+  int ci = (cc * KG + kg) * 8 + jj;
+  float v = 0.0f;
+  if (ci < cin_pad) v = wt[((size_t)tap * cin_pad + ci) * cout_pad + nt * NT + n];
+  w[i] = __float2half_rn(v);
+}
 
 }  // namespace tc
+
+// channel groups (16 bytes: 4 fp32 or 8 fp16 channels) per chunk of a convolution with G input groups
+static int conv_tc_kg(int ntaps, int NT, int G) {
+  int KG = (ntaps == 27 && NT > 64) ? 4 : 8;
+  if (G < KG) KG = (G <= 2) ? 2 : ((G <= 4) ? 4 : 8);
+  return KG;
+}
 
 // The tiling of a convolution: decided here once, stored in w.tc with the packing laid out for it, and read by
 // conv_tc_run, ygemm and sa_fused.  Adds the step that packs w.wt into w.tc.w.
@@ -645,14 +683,37 @@ int conv_tc_prepare(Model* m, ConvW& w) {
   // round trip is amortised over more MMAs -- and 16-channel chunks for N = 128, where the 9-tap
   // weight slab (2 x 72 KB) leaves room for a 16-channel ring only.
   // 1x1: 32-channel chunks.
-  t.KG = (w.ntaps == 27 && t.NT > 64) ? 4 : 8;
-  if (G < t.KG) t.KG = (G <= 2) ? 2 : ((G <= 4) ? 4 : 8);
+  t.KG = conv_tc_kg(w.ntaps, t.NT, G);
   t.nchunk = (G + t.KG - 1) / t.KG;
   const size_t total = (size_t)(w.cout_pad / t.NT) * t.nchunk * t.ntg * t.tpg * t.KG * t.NT * 4;
   LION_TRY(m->dmalloc(&t.w, total));
   w.tc = t;
   m->repack.push_back([t, wt = w.wt, ntaps = w.ntaps, cin_pad = w.cin_pad, cout_pad = w.cout_pad, total] {
     tc::k_pack_tc<<<(unsigned)cdivz(total, 256), 256>>>(wt, t.w, ntaps, cin_pad, cout_pad, t.NT, t.nchunk, t.ntg, t.tpg, t.KG);
+  });
+  return 0;
+}
+
+// The FP16 tiling of a 3x3x3 convolution that has a TF32 one: the same record in 16-byte groups (C/8 of them), so KG,
+// the chunk bytes, the rings, the block groups and the work distribution follow from bytes exactly as for TF32.  Only
+// the cases the second convolutions of the PVConvs use are compiled (conv_tc_run), and only those are served: Cin = Cout =
+// 32, 64 or 128 (N = 32, 64, 128 with KG = 4, 8, 4).  Allocates and adds the packing step; the caller runs it.  A
+// convolution the FP16 kernels do not serve keeps tc16.w == nullptr.
+int conv_tc_prepare_f16(Model* m, ConvW& w) {
+  if (w.tc16.w || !w.tc.w || w.ntaps != 27 || w.cin_pad != w.cout_pad || w.cout != w.cout_pad) return 0;
+  if (!(w.cout_pad == 32 || w.cout_pad == 64 || w.cout_pad == 128)) return 0;
+  ConvTcW t = w.tc;
+  const int G = w.cin_pad / 8;
+  t.KG = conv_tc_kg(w.ntaps, t.NT, G);
+  t.nchunk = (G + t.KG - 1) / t.KG;
+  if (!((t.NT == 32 && t.KG == 4) || (t.NT == 64 && t.KG == 8) || (t.NT == 128 && t.KG == 4))) return 0;
+  const size_t total = (size_t)(w.cout_pad / t.NT) * t.nchunk * t.ntg * t.tpg * t.KG * t.NT * 8;
+  __half* w16 = nullptr;
+  LION_TRY(m->dmalloc(&w16, total));
+  t.w = reinterpret_cast<float*>(w16);
+  w.tc16 = t;
+  m->repack.push_back([t, w16, wt = w.wt, ntaps = w.ntaps, cin_pad = w.cin_pad, cout_pad = w.cout_pad, total] {
+    tc::k_pack_tc16<<<(unsigned)cdivz(total, 256), 256>>>(wt, w16, ntaps, cin_pad, cout_pad, t.NT, t.nchunk, t.ntg, t.tpg, t.KG);
   });
   return 0;
 }
@@ -664,17 +725,19 @@ bool conv_tc_usable(const ConvW& w, const ConvGeom& geo) {
 }
 
 int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, double* ssum, double* ssq,
-                const ConvGeom& geo, int B, float* pool_mm) {
+                const ConvGeom& geo, int B, float* pool_mm, bool f16) {
   tc::Params P{};
+  if (f16 && !w.tc16.w) { set_error("conv_tc: no FP16 packing of this convolution"); return LION_ERR_STATE; }
+  const ConvTcW& T = f16 ? w.tc16 : w.tc;   // f16: the input is [C/8][rows][8] halves
   if (pool_mm && (w.ntaps != 1 || geo.p_begin != 0 || geo.p_end != geo.rows || geo.rows % 128)) {
     set_error("conv_tc: the pooled epilogue needs a 1x1 convolution over a multiple of 128 rows"); return LION_ERR_ARG;
   }
   P.pool_mm = pool_mm;
-  const int NT = w.tc.NT, KG = w.tc.KG, tpg = w.tc.tpg;
-  P.in = in; P.w = w.tc.w; P.bias = w.bias; P.out = out; P.ssum = ssum; P.ssq = ssq;
+  const int NT = T.NT, KG = T.KG, tpg = T.tpg;
+  P.in = in; P.w = T.w; P.bias = w.bias; P.out = out; P.ssum = ssum; P.ssq = ssq;
   P.Gin = Gin; P.Gout_store = Gout_store; P.cout_pad = w.cout_pad;
   P.rows = geo.rows; P.p_begin = geo.p_begin; P.p_end = geo.p_end;
-  P.ntg = w.tc.ntg; P.tpg = tpg; P.KG = KG; P.nchunk = w.tc.nchunk; P.NT = NT;
+  P.ntg = T.ntg; P.tpg = tpg; P.KG = KG; P.nchunk = T.nchunk; P.NT = NT;
   const int slab_bytes = tpg * KG * NT * 16;     // the weights of one (channel chunk, x-plane)
   P.B = B;
   P.occ = geo.occ; P.occ_stride = geo.occ_stride;
@@ -823,25 +886,31 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   const int bpw = blk ? P.ib / 2 : 1;
   c->conv_group_blocks = blk ? P.ib : 0;
   c->conv_stage_taps = P.tps;
-#define CONV_TC_CASE(kg, tpg_, nt_, blk_, bpw_, tps_)                                                     \
-  if (KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_ && bpw == bpw_ && P.tps == tps_) {              \
+#define CONV_TC_CASE_OP(kg, tpg_, nt_, blk_, bpw_, tps_, op)                                              \
+  if (f16 == std::is_same<op, __half>::value && KG == kg && tpg == tpg_ && NT == nt_ && blk == blk_ && bpw == bpw_ && P.tps == tps_) { \
     static DevOnce attr_once;                                                                             \
     if (attr_once.need()) {                                                                               \
-      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
+      LION_CHECK_CUDA(cudaFuncSetAttribute(tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_, op>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
     }                                                                                                     \
-    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_>), grid, tc::conv_threads(bpw_), smem, P); \
+    LION_LAUNCH(c, (tc::k_conv_tc<kg, tpg_, nt_, blk_, bpw_, tps_, op>), grid, tc::conv_threads(bpw_), smem, P); \
     LION_TRY(check_launch(c, "conv_tc"));                                                                 \
     return stats();                                                                                       \
   }
+#define CONV_TC_CASE(kg, tpg_, nt_, blk_, bpw_, tps_) CONV_TC_CASE_OP(kg, tpg_, nt_, blk_, bpw_, tps_, float)
 #define CONV_TC_NT(kg, tpg_) CONV_TC_CASE(kg, tpg_, 32, false, 1, tpg_) CONV_TC_CASE(kg, tpg_, 64, false, 1, tpg_) CONV_TC_CASE(kg, tpg_, 96, false, 1, tpg_)
 #define CONV_TC_BLK(kg, bpw_) CONV_TC_CASE(kg, 9, 128, true, bpw_, 9) CONV_TC_CASE(kg, 9, 128, true, bpw_, 3)
   CONV_TC_NT(2, 1) CONV_TC_NT(4, 1) CONV_TC_NT(8, 1) CONV_TC_NT(2, 9) CONV_TC_NT(4, 9) CONV_TC_NT(8, 9)
   CONV_TC_CASE(2, 1, 128, false, 1, 1) CONV_TC_CASE(4, 1, 128, false, 1, 1) CONV_TC_CASE(8, 1, 128, false, 1, 1)
   CONV_TC_BLK(2, 1) CONV_TC_BLK(4, 1) CONV_TC_BLK(2, 2) CONV_TC_BLK(4, 2)
+  // FP16 operands: the second convolutions of the PVConvs only (conv_tc_prepare_f16)
+  CONV_TC_CASE_OP(4, 9, 32, false, 1, 9, __half) CONV_TC_CASE_OP(8, 9, 64, false, 1, 9, __half)
+  CONV_TC_CASE_OP(4, 9, 128, true, 1, 9, __half) CONV_TC_CASE_OP(4, 9, 128, true, 1, 3, __half)
+  CONV_TC_CASE_OP(4, 9, 128, true, 2, 9, __half) CONV_TC_CASE_OP(4, 9, 128, true, 2, 3, __half)
 #undef CONV_TC_NT
 #undef CONV_TC_BLK
 #undef CONV_TC_CASE
-  set_error("conv_tc: no kernel for N=%d, KG=%d, %d taps, %d per weight stage", NT, KG, tpg, P.tps);
+#undef CONV_TC_CASE_OP
+  set_error("conv_tc: no %s kernel for N=%d, KG=%d, %d taps, %d per weight stage", f16 ? "FP16" : "TF32", NT, KG, tpg, P.tps);
   return LION_ERR_ARG;
 }
 

@@ -12,9 +12,9 @@ struct StyleLayer { const float* w; const float* b; int n_out; int out_off; };
 // tensor-core packing of a convolution's weights and the tiling it is packed for (conv_tc_prepare);
 // w == nullptr -> SIMT kernel only
 struct ConvTcW {
-  float* w = nullptr;    // [n-tile][chunk][tap group][tap][KG][NT][4], tf32-rounded
+  float* w = nullptr;    // [n-tile][chunk][tap group][tap][KG][NT][4], tf32-rounded (tc16: [...][NT][8] fp16 bits)
   int NT = 0;            // output channels per CTA (wgmma N, <= 128)
-  int KG = 0;            // 4-channel input groups per pipeline chunk (2, 4 or 8)
+  int KG = 0;            // 16-byte input groups (4 fp32 / 8 fp16 channels) per pipeline chunk (2, 4 or 8)
   int nchunk = 0;        // chunks
   int ntg = 0, tpg = 0;  // tap groups (x planes) and taps per group: (3, 9) or (1, 1)
 };
@@ -34,6 +34,7 @@ struct ConvW {
   float* wt = nullptr;      // [ntaps][cin_pad][cout_pad]   (SIMT kernel)
   float* bias = nullptr;    // [cout_pad]
   ConvTcW tc;               // tensor-core packing (conv_tc.cuh); tc.w == nullptr when unsupported
+  ConvTcW tc16;             // FP16 packing and tiling (conv_tc_prepare_f16, made on the first FP16 forward) or w == nullptr
 };
 struct AdaGNW {
   const float* gamma = nullptr; const float* beta = nullptr;
@@ -116,6 +117,7 @@ struct Model {
   // Run once at build and again by lion_model_refresh after the parameters changed in place.  A step captures device
   // pointers and sizes by value: the ConvWs it serves live in vectors that may still grow while the model is built.
   std::vector<std::function<void()>> repack;
+  bool f16_ready = false;      // the FP16 packings exist (ensure_f16 in net.cu)
   std::vector<StyleLayer> style_layers;
   StyleLayer* d_style_layers = nullptr;
   int style_total = 0;
@@ -172,6 +174,7 @@ struct ConvGeom {
 
 // conv_tc.cu
 int conv_tc_prepare(Model* m, ConvW& w);
+int conv_tc_prepare_f16(Model* m, ConvW& w);
 bool conv_tc_usable(const ConvW& w, const ConvGeom& geo);
 // sparse first convolution, GEMM half (sparse_conv.cu)
 bool ygemm_usable(const ConvW& y);
@@ -182,6 +185,6 @@ int sa_fused_run(Ctx* c, const SABlk& s, const float4* feat, const float4* point
                  const float* scale1, const float* shift1, double* ssum, double* ssq, int stat_stride, float* pool_mm,
                  int B, int N);
 int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, double* ssum,
-                double* ssq, const ConvGeom& geo, int B, float* pool_mm = nullptr);
+                double* ssq, const ConvGeom& geo, int B, float* pool_mm = nullptr, bool f16 = false);
 
 }  // namespace lion

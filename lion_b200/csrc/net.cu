@@ -149,6 +149,34 @@ int run_repack(Model* m) {
   return 0;
 }
 
+// The FP16 packings of the convolutions an FP16 forward uses (the second convolution of every PVConv, or a stand-alone
+// Conv3d), made on the model's first FP16 forward: allocated, packed now, and re-packed by lion_model_refresh with the
+// TF32 ones.  Allocation is not capturable: the first FP16 call must be eager (the samplers' first step is).
+static int ensure_f16(Model* m, void* stream) {
+  // the context's mutex: the first FP16 calls of two threads, or one and a lion_model_refresh, must not both append to
+  // m->repack or pack tc16
+  std::unique_lock<std::mutex> lock;
+  if (m->ctx->mu) lock = std::unique_lock<std::mutex>(*m->ctx->mu);
+  if (m->f16_ready) return 0;
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  cudaStreamIsCapturing((cudaStream_t)stream, &st);
+  LION_REQUIRE(st == cudaStreamCaptureStatusNone, "FP16 forward: the model's first FP16 call must run outside stream capture");
+  LION_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  const size_t first = m->repack.size();
+  auto pv = [&](std::vector<std::vector<Block>>& levels) -> int {
+    for (auto& lv : levels) for (auto& b : lv) if (b.kind == LION_KIND_PVCONV) LION_TRY(conv_tc_prepare_f16(m, b.pv.c2));
+    return 0;
+  };
+  if (m->unet) { LION_TRY(pv(m->unet->sa)); LION_TRY(pv(m->unet->fp)); }
+  if (m->block && m->block->kind == LION_KIND_PVCONV) LION_TRY(conv_tc_prepare_f16(m, m->block->pv.c2));
+  if (m->kind == LION_KIND_CONV3D) LION_TRY(conv_tc_prepare_f16(m, m->conv_single));
+  for (size_t i = first; i < m->repack.size(); ++i) m->repack[i]();
+  LION_CHECK_CUDA(cudaGetLastError());
+  LION_CHECK_CUDA(cudaDeviceSynchronize());
+  m->f16_ready = true;
+  return 0;
+}
+
 // plain: nn.GroupNorm(8, C) of the non-Ada blocks (models/pvcnn2.py) = AdaGN whose style Linear is identically
 // (factor, bias) = (1, 0): no `emd` parameters are consumed and k_style_linear writes the constants.
 int make_adagn(Model* m, AdaGNW& g, Cursor& cur, int C, bool plain = false) {
@@ -259,6 +287,7 @@ struct MlpRecord {
 // so that a read of a halo row nobody wrote shows up instead of depending on what the arena held.
 struct PvRecord {
   const float4 *raw1 = nullptr, *act1 = nullptr, *raw2 = nullptr;   // VGs of cout channels (act1: halo included)
+  bool act1_f16 = false;          // act1 holds rows of 8 halves (FP16 second convolution)
   const float4 *rawp = nullptr, *fused = nullptr;                    // PFs: point-branch 1x1 output, devox + point branch
   AffSrc a1{}, ap{}, a2{};        // AdaGN-1, point-branch AdaGN, AdaGN-2 with the SE gate: sums and folded scale / shift
   int conv2 = -1;                 // 0 = SIMT, 1 = tensor-core row tiles, 2 / 4 = interior-block groups of that many blocks
@@ -272,6 +301,7 @@ struct Fwd {
   std::deque<VoxPrep> vox;       // a deque: get_vox hands out pointers that later preps must not move
   MlpRecord* rec = nullptr;      // test entry points only
   PvRecord* pv = nullptr;        // test entry points only
+  bool conv_f16 = false;         // LION_FWD_CONV_FP16: the PVConvs' second convolutions take FP16 operands (pvconv_fwd)
 };
 static void record_layer(Fwd& f, const AffSrc& a) {
   MlpRecord* r = f.rec;
@@ -339,9 +369,12 @@ static ConvGeom geom_grid(int r) {
 }
 
 // out rows in [p_begin,p_end) of every (b, group < Gout_store); statistics optional
+// f16: the input is [Gin = C/8][rows][8] halves and the FP16 kernel runs (w.tc16 must exist)
 static int run_conv(Fwd& f, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store,
-                    double* ssum, double* ssq, const ConvGeom& geo, float* pool_mm = nullptr) {
-  if (Gin * 4 != w.cin_pad) { set_error("conv: input has %d channels, weights expect %d", Gin * 4, w.cin_pad); return LION_ERR_ARG; }
+                    double* ssum, double* ssq, const ConvGeom& geo, float* pool_mm = nullptr, bool f16 = false) {
+  const int cpg = f16 ? 8 : 4;
+  if (Gin * cpg != w.cin_pad) { set_error("conv: input has %d channels, weights expect %d", Gin * cpg, w.cin_pad); return LION_ERR_ARG; }
+  if (f16) return conv_tc_run(f.c, w, in, Gin, out, Gout_store, ssum, ssq, geo, f.B, pool_mm, true);
   if (conv_tc_usable(w, geo))
     return conv_tc_run(f.c, w, in, Gin, out, Gout_store, ssum, ssq, geo, f.B, pool_mm);
   if (pool_mm) { set_error("conv: the pooled epilogue exists on the tensor-core path only"); return LION_ERR_STATE; }
@@ -407,10 +440,10 @@ static int alloc_stats(Fwd& f, int stride, double** ssum, double** ssq) {
 // code on the critical path loses to a 32-CTA kernel whose launch latency the graph mostly hides -- so the separate
 // launch stays.
 static int conv_gn(Fwd& f, const ConvW& w, const float4* in, int Gin, float4* out, int Gout_store, const ConvGeom& geo,
-                   const AdaGNW& g, double count, const float* se1, const float* se2, AffSrc& a) {
+                   const AdaGNW& g, double count, const float* se1, const float* se2, AffSrc& a, bool f16 = false) {
   double *ssum, *ssq;
   LION_TRY(alloc_stats(f, w.cout_pad, &ssum, &ssq));
-  LION_TRY(run_conv(f, w, in, Gin, out, Gout_store, ssum, ssq, geo));
+  LION_TRY(run_conv(f, w, in, Gin, out, Gout_store, ssum, ssq, geo, nullptr, f16));
   return run_affine(f, g, ssum, ssq, w.cout_pad, count, se1, se2, a);
 }
 // same, but the fold is left to the caller (who merges it with another layer's: run_prep)
@@ -569,7 +602,8 @@ static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, 
       // cannot become resident on the SMs FPS occupies (see unet_forward)
       LION_CHECK_CUDA(cudaFuncSetAttribute(k_sparse_conv_gather<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
       LION_CHECK_CUDA(cudaFuncSetAttribute(k_sparse_conv_gather<64>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-      LION_CHECK_CUDA(cudaFuncSetAttribute(k_act_grid, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      LION_CHECK_CUDA(cudaFuncSetAttribute(k_act_grid<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      LION_CHECK_CUDA(cudaFuncSetAttribute(k_act_grid<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
       LION_CHECK_CUDA(cudaFuncSetAttribute(k_scatter_compact, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
     const dim3 grid(cdiv(r * r * r, 32 * nwarp), f.B);
@@ -614,24 +648,30 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   stamp(f.c, f.c->stream, " conv1");
   // AdaGN-1 + Swish as a stand-alone pass over the grid (HBM-bound).  Folding it into conv2's operand staging
   // ("transform on load") was parity-green but made the convolutions 3.5x slower (measured on the B200, before the
-  // port to H100).  Its extra blocks re-zero the scatter grid (was: k_unscatter).
-  float4* act1 = alloc_vg(f, Gout, r);
-  LION_TRY(poison_vg(f, act1, Gout, r));
+  // port to H100).  Its extra blocks re-zero the scatter grid (was: k_unscatter).  FP16 mode (where the FP16 kernel
+  // serves conv2): the grid is [C/8][P][8] halves, half the bytes, and conv2 takes FP16 operands.
+  const bool h2 = f.conv_f16 && p.c2.tc16.w;
+  const int Gact = h2 ? Gout / 2 : Gout;
+  float4* act1 = alloc_vg(f, Gact, r);
+  LION_TRY(poison_vg(f, act1, Gact, r));
   {
     const int nb_act = cdiv(P, 256 * ACT_U);
-    LION_LAUNCH(f.c, k_act_grid, dim3(nb_act + (sparse1 ? 0 : cdiv(N, 256)), Gout, f.B), 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act,
-                vp->ppos, g_in, Gin, N);
+    const dim3 grid(nb_act + (sparse1 ? 0 : cdiv(N, 256)), Gact, f.B);
+    if (h2)
+      LION_LAUNCH(f.c, k_act_grid<true>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N);
+    else
+      LION_LAUNCH(f.c, k_act_grid<false>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N);
   }
   stamp(f.c, f.c->stream, " act1");
   // conv2 -> (stats) -> AdaGN + SE folded into one affine
   float4* raw2 = alloc_vg(f, Gout, r);
   LION_TRY(poison_vg(f, raw2, Gout, r));
   AffSrc a2;
-  LION_TRY(conv_gn(f, p.c2, act1, Gout, raw2, Gout, geo, p.g2, V, p.se1, p.se2, a2));
+  LION_TRY(conv_gn(f, p.c2, act1, Gact, raw2, Gout, geo, p.g2, V, p.se1, p.se2, a2, h2));
   stamp(f.c, f.c->stream, " conv2");
   if (f.pv) {
     PvRecord& R = *f.pv;
-    R.raw1 = raw1; R.act1 = act1; R.raw2 = raw2; R.rawp = rawp.p;
+    R.raw1 = raw1; R.act1 = act1; R.raw2 = raw2; R.rawp = rawp.p; R.act1_f16 = h2;
     R.a1 = a1; R.ap = ap; R.a2 = a2;
     R.conv2 = !conv_tc_usable(p.c2, geo) ? 0 : f.c->conv_group_blocks ? f.c->conv_group_blocks : 1;
   }
@@ -1304,16 +1344,24 @@ extern "C" int lion_model_create(LionCtx* ctx, int kind, const int* desc, int nd
 extern "C" int lion_model_destroy(LionModel* h) { delete h; return 0; }
 extern "C" int lion_model_refresh(LionModel* h) {
   LION_REQUIRE(h, "lion_model_refresh: null model");
+  std::unique_lock<std::mutex> lock;                     // (ensure_f16 may be appending FP16 packing steps)
+  if (h->m.ctx->mu) lock = std::unique_lock<std::mutex>(*h->m.ctx->mu);
   LION_CHECK_CUDA(cudaSetDevice(h->m.ctx->device));
   return run_repack(&h->m);
 }
 
 extern "C" int lion_unet_forward(LionModel* h, const float* x, const float* t, const float* style, const float* clip,
                                  float* out, int B, int N, void* stream) {
+  return lion_unet_forward_flags(h, x, t, style, clip, out, B, N, 0, stream);
+}
+extern "C" int lion_unet_forward_flags(LionModel* h, const float* x, const float* t, const float* style, const float* clip,
+                                       float* out, int B, int N, int flags, void* stream) {
   LION_REQUIRE(h && h->m.kind == LION_KIND_UNET, "lion_unet_forward: not a unet model");
-  LION_REQUIRE(x && out && B > 0 && N > 0, "lion_unet_forward: bad arguments");
+  LION_REQUIRE(x && out && B > 0 && N > 0 && (flags & ~LION_FWD_CONV_FP16) == 0, "lion_unet_forward: bad arguments");
   Model* m = &h->m;
-  return two_pass(m, stream, B, [&](Fwd& f) { return unet_forward(f, x, t, style, clip, out, N); });
+  const bool f16 = (flags & LION_FWD_CONV_FP16) != 0;
+  if (f16) LION_TRY(ensure_f16(m, stream));
+  return two_pass(m, stream, B, [&](Fwd& f) { f.conv_f16 = f16; return unet_forward(f, x, t, style, clip, out, N); });
 }
 
 extern "C" int lion_style_encoder_forward(LionModel* h, const float* x, float* out, int B, int N, void* stream) {
@@ -1503,21 +1551,32 @@ extern "C" int lion_swish_fwd(const float* x, float* out, size_t n, void* stream
 // ---- stand-alone Conv3d 3x3x3 + fused GroupNorm statistics (reference: nn.Conv3d in
 // models/pvcnn2_ada.py:211-222 followed by AdaGN's GroupNorm, models/adagn.py:36) -----------------
 extern "C" int lion_conv3d_gn_fwd(LionModel* h, const float* x, float* out, double* gn_sum, double* gn_sqsum, int B, void* stream) {
+  return lion_conv3d_gn_fwd_flags(h, x, out, gn_sum, gn_sqsum, B, 0, stream);
+}
+extern "C" int lion_conv3d_gn_fwd_flags(LionModel* h, const float* x, float* out, double* gn_sum, double* gn_sqsum, int B,
+                                        int flags, void* stream) {
   LION_REQUIRE(h && h->m.kind == LION_KIND_CONV3D, "lion_conv3d_gn_fwd: not a conv3d model");
-  LION_REQUIRE(x && out && B > 0 && ((gn_sum == nullptr) == (gn_sqsum == nullptr)), "lion_conv3d_gn_fwd: bad arguments");
+  LION_REQUIRE(x && out && B > 0 && ((gn_sum == nullptr) == (gn_sqsum == nullptr)) && (flags & ~LION_FWD_CONV_FP16) == 0,
+               "lion_conv3d_gn_fwd: bad arguments");
   Model* m = &h->m;
+  if (flags & LION_FWD_CONV_FP16) LION_TRY(ensure_f16(m, stream));
+  // FP16 where the FP16 kernel serves the shape; otherwise exactly the TF32 call
+  const bool f16 = (flags & LION_FWD_CONV_FP16) && m->conv_single.tc16.w;
   return two_pass(m, stream, B, [&](Fwd& f) -> int {
     const ConvW& w = m->conv_single;
     const int cin = m->desc[0], cout = m->desc[1], r = m->desc[2];
-    const int Gin = w.cin_pad / 4, Gout = (cout + 3) / 4, rp = r + 2, V = r * r * r;
+    const int Gin = w.cin_pad / (f16 ? 8 : 4), Gout = (cout + 3) / 4, rp = r + 2, V = r * r * r;
     const size_t P = (size_t)rp * rp * rp;
     float4* gi = alloc_vg(f, Gin, r);
     LION_TRY(memset_async(f.c, gi, 0, sizeof(float4) * (size_t)B * Gin * P));
-    LION_LAUNCH(f.c, k_cm_to_vg, dim3(cdiv(V, 256), Gin, B), 256, 0, x, gi, cin, Gin, r, 1);
+    if (f16)
+      LION_LAUNCH(f.c, k_cm_to_vg_h8, dim3(cdiv(V, 256), Gin, B), 256, 0, x, gi, cin, Gin, r);
+    else
+      LION_LAUNCH(f.c, k_cm_to_vg, dim3(cdiv(V, 256), Gin, B), 256, 0, x, gi, cin, Gin, r, 1);
     float4* go = alloc_vg(f, Gout, r);
     double *ssum = nullptr, *ssq = nullptr;
     if (gn_sum) LION_TRY(alloc_stats(f, w.cout_pad, &ssum, &ssq));
-    LION_TRY(run_conv(f, w, gi, Gin, go, Gout, ssum, ssq, geom_grid(r)));
+    LION_TRY(run_conv(f, w, gi, Gin, go, Gout, ssum, ssq, geom_grid(r), nullptr, f16));
     LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(V, 256), Gout, B), 256, 0, go, out, cout, Gout, r);
     if (gn_sum && !f.c->dry) {
       LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sum, sizeof(double) * cout, ssum, sizeof(double) * w.cout_pad, sizeof(double) * cout, B,
@@ -1549,7 +1608,7 @@ extern "C" int lion_pvconv_conv1_probe(LionModel* h, const float* features, cons
     LION_TRY(pvconv_conv1(f, p, x, vp, path, c1, [] { return 0; }));
     // the dense path scattered into the context's zero grid: zero those voxels again (k_act_grid's extra blocks alone)
     if (!c1.sparse)
-      LION_LAUNCH(f.c, k_act_grid, dim3(cdiv(N, 256), Gout, B), 256, 0, c1.raw, nullptr, AffSrc{}, Gout, p.cout, rp, P, 0,
+      LION_LAUNCH(f.c, k_act_grid<false>, dim3(cdiv(N, 256), Gout, B), 256, 0, c1.raw, nullptr, AffSrc{}, Gout, p.cout, rp, P, 0,
                   vp->ppos, c1.g_in, p.cin / 4, N);
     LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), Gout, B), 256, 0, c1.raw, out, p.cout, Gout, r);
     if (!f.c->dry) {
@@ -1623,15 +1682,25 @@ extern "C" int lion_sa_mlp_probe(LionModel* h, const float* features, const floa
 extern "C" int lion_pvconv_probe(LionModel* h, const float* features, const float* coords, const float* style, float* raw1,
                                  float* act1, float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out,
                                  int* conv2_kernel, int B, int N, void* stream) {
+  return lion_pvconv_probe_flags(h, features, coords, style, raw1, act1, raw2, rawp, sums, affine, fused, out, conv2_kernel, B, N,
+                                 0, stream);
+}
+// flags LION_FWD_CONV_FP16: act1 is the FP16 grid (where the FP16 kernel serves conv2), returned widened to fp32
+extern "C" int lion_pvconv_probe_flags(LionModel* h, const float* features, const float* coords, const float* style, float* raw1,
+                                       float* act1, float* raw2, float* rawp, double* sums, float* affine, float* fused, float* out,
+                                       int* conv2_kernel, int B, int N, int flags, void* stream) {
   LION_REQUIRE(h && h->m.kind == LION_KIND_PVCONV, "lion_pvconv_probe: not a pvconv model");
   LION_REQUIRE(features && coords && (style || h->m.desc[4] == 0) && raw1 && act1 && raw2 && rawp && sums && affine && fused &&
-               out && B > 0 && N > 0, "lion_pvconv_probe: bad arguments");
+               out && B > 0 && N > 0 && (flags & ~LION_FWD_CONV_FP16) == 0, "lion_pvconv_probe: bad arguments");
   Model* m = &h->m;
+  const bool f16 = (flags & LION_FWD_CONV_FP16) != 0;
+  if (f16) LION_TRY(ensure_f16(m, stream));
   return two_pass(m, stream, B, [&](Fwd& f) -> int {
     const PVConvBlk& p = m->block->pv;
     const int C = p.cout, G = C / 4, r = p.r, rp = r + 2;
     PvRecord rec;
     f.pv = &rec;
+    f.conv_f16 = f16;
     LION_TRY(style_affine_all(f, style ? style : f.c->alloc_n<float>((size_t)B * 4)));
     PF x = to_pf(f, features, m->desc[0], N);
     float4* c4 = to_c4(f, coords, N);
@@ -1639,7 +1708,10 @@ extern "C" int lion_pvconv_probe(LionModel* h, const float* features, const floa
     LION_TRY(pvconv_fwd(f, p, x, c4, o.p, o.G, 0));
     // (the arena pvconv_fwd released is not reused before these copies: they are the next work on the stream)
     LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), G, B), 256, 0, rec.raw1, raw1, C, G, r);
-    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(rp * rp * rp, 256), G, B), 256, 0, rec.act1, act1, C, G, rp * rp * rp);
+    if (rec.act1_f16)
+      LION_LAUNCH(f.c, k_h8_to_cm, dim3(cdiv(rp * rp * rp, 256), G / 2, B), 256, 0, rec.act1, act1, C, G / 2, rp * rp * rp);
+    else
+      LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(rp * rp * rp, 256), G, B), 256, 0, rec.act1, act1, C, G, rp * rp * rp);
     LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), G, B), 256, 0, rec.raw2, raw2, C, G, r);
     LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.rawp, rawp, C, G, N);
     LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.fused, fused, C, G, N);

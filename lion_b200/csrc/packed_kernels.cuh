@@ -12,6 +12,7 @@
 // into 27 constant row offsets (implicit GEMM without im2col or bounds checks), which is what
 // the wgmma kernel (conv_tc.cu) exploits with shifted shared-memory operand descriptors.
 #pragma once
+#include <cuda_fp16.h>
 #include "common.cuh"
 #include "point_core.cuh"
 #include "model.cuh"
@@ -592,11 +593,25 @@ __device__ __forceinline__ void aff_block_load(const AffSrc& a, int b, int g, in
 // ACT_U positions per thread, loads issued before any use: a 16-byte access per thread leaves too
 // few bytes in flight per SM to cover HBM latency (4.3 TB/s measured with one access per thread).
 constexpr int ACT_U = 4;
+// 8 floats -> one 16-byte row of 8 halves, each rounded to nearest even
+__device__ __forceinline__ float4 h8_pack(float4 a, float4 b) {
+  union { __half2 h[4]; float4 f; } u;
+  u.h[0] = __floats2half2_rn(a.x, a.y); u.h[1] = __floats2half2_rn(a.z, a.w);
+  u.h[2] = __floats2half2_rn(b.x, b.y); u.h[3] = __floats2half2_rn(b.z, b.w);
+  return u.f;
+}
+
+// The output form F16 (the input of the FP16 second convolution): block (x, y, b) covers channels 8y .. 8y + 7, i.e. fp32
+// groups 2y and 2y + 1 of `in` (G of them), applies the same affine and Swish in fp32 and stores one row of 8 halves
+// (rounded to nearest even) per position into out [B][G/2][P][8].  Otherwise block (x, y, b) covers group y and stores
+// the TF32-rounded float4 into out [B][G][P][4].  Halo positions are exactly 0 in both forms.
 // Blocks with blockIdx.x >= nb_act do k_unscatter's job instead (us_ppos != null): they restore the all-zero
 // invariant of the persistent scatter grid that the first convolution has finished reading by now (one launch less
 // per PVConv on the critical path); block (x, y, z) zeroes its 256 points in groups y, y + gridDim.y, ... < us_G.
+template <bool F16>
 __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ out, AffSrc aff, int G, int C, int rp, int P,
                            int nb_act, const int* __restrict__ us_ppos, float4* __restrict__ us_grid, int us_G, int us_N) {
+  constexpr int NG = F16 ? 2 : 1;                       // fp32 input groups per output row
   int b = blockIdx.z, g = blockIdx.y;
   if ((int)blockIdx.x >= nb_act) {
     int sidx = ((int)blockIdx.x - nb_act) * blockDim.x + threadIdx.x;
@@ -606,12 +621,16 @@ __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ o
       for (int gg = g; gg < us_G; gg += gridDim.y) us_grid[((size_t)b * us_G + gg) * P + pp] = make_float4(0.f, 0.f, 0.f, 0.f);
     return;
   }
-  float4 s, t;
-  aff_block_load(aff, b, g, C, s, t);
-  const float4* src = in + ((size_t)b * G + g) * P;
-  float4* dst = out + ((size_t)b * G + g) * P;
+  float4 s[NG], t[NG];
+#pragma unroll
+  for (int k = 0; k < NG; ++k) {
+    if (k) __syncthreads();                              // (aff_block_load's shared slots are reused)
+    aff_block_load(aff, b, NG * g + k, C, s[k], t[k]);
+  }
+  const float4* src = in + ((size_t)b * G + NG * g) * P;
+  float4* dst = out + ((size_t)b * (G / NG) + g) * P;
   const int p0 = blockIdx.x * (blockDim.x * ACT_U) + threadIdx.x;
-  float4 v[ACT_U];
+  float4 v[ACT_U][NG];
   bool interior[ACT_U];
   // p -> (x, y, z) by multiply-high with m = ceil(2^32 / rp) (exact while p * rp < 2^32): the four positions of a thread
   // cost one integer division instead of sixteen -- at 1 float4 per clock per SM this pass is instruction-bound, not
@@ -623,15 +642,21 @@ __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ o
     const int q = (int)__umulhi((unsigned)p, rp_m), x = (int)__umulhi((unsigned)q, rp_m);
     const int z = p - q * rp, y = q - x * rp;
     interior[u] = p < P && z >= 1 && z <= rp - 2 && y >= 1 && y <= rp - 2 && x >= 1 && x <= rp - 2;
-    v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (interior[u]) v[u] = __ldcs(src + p);          // read once: streaming
+#pragma unroll
+    for (int k = 0; k < NG; ++k) {
+      v[u][k] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (interior[u]) v[u][k] = __ldcs(src + (size_t)k * P + p);   // read once: streaming
+    }
   }
 #pragma unroll
   for (int u = 0; u < ACT_U; ++u) {
     int p = p0 + u * blockDim.x;
     if (p < P) {
       float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (interior[u]) r = f4_tf32(f4_swish(f4_affine(v[u], s, t)));   // sole consumer: the second 3x3x3 convolution
+      if (interior[u]) {                                 // sole consumer: the second 3x3x3 convolution
+        if constexpr (F16) r = h8_pack(f4_swish(f4_affine(v[u][0], s[0], t[0])), f4_swish(f4_affine(v[u][1], s[1], t[1])));
+        else r = f4_tf32(f4_swish(f4_affine(v[u][0], s[0], t[0])));
+      }
       dst[p] = r;
     }
   }
@@ -1040,6 +1065,35 @@ __global__ void k_cm_to_vg(const float* __restrict__ src, float4* __restrict__ d
   float4 o = make_float4(v[0], v[1], v[2], v[3]);
   if (tf32) o = f4_tf32(o);
   dst[((size_t)b * G + g) * ((size_t)rp * rp * rp) + prow] = o;
+}
+// the FP16 form of k_cm_to_vg: dst [B][G8][(r+2)^3] rows of 8 halves (channels 8 g8 .. 8 g8 + 7, rounded to nearest even)
+__global__ void k_cm_to_vg_h8(const float* __restrict__ src, float4* __restrict__ dst, int C, int G8, int r) {
+  int b = blockIdx.z, g = blockIdx.y;
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  int V = r * r * r, rp = r + 2;
+  if (i >= V) return;
+  int x = i / (r * r), y = (i / r) % r, z = i % r;
+  size_t prow = ((size_t)(x + 1) * rp + (y + 1)) * rp + (z + 1);
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    int c = g * 8 + j;
+    v[j] = c < C ? src[((size_t)b * C + c) * V + i] : 0.0f;
+  }
+  dst[((size_t)b * G8 + g) * ((size_t)rp * rp * rp) + prow] = h8_pack(make_float4(v[0], v[1], v[2], v[3]), make_float4(v[4], v[5], v[6], v[7]));
+}
+// rows of 8 halves [B][G8][R] -> channel-major fp32 [B][C][R] (exact)
+__global__ void k_h8_to_cm(const float4* __restrict__ src, float* __restrict__ dst, int C, int G8, int R) {
+  int b = blockIdx.z, g = blockIdx.y;
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R) return;
+  union { float4 f; __half h[8]; } u;
+  u.f = src[((size_t)b * G8 + g) * R + i];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    int c = g * 8 + j;
+    if (c < C) dst[((size_t)b * C + c) * R + i] = __half2float(u.h[j]);
+  }
 }
 __global__ void k_vg_to_cm(const float4* __restrict__ src, float* __restrict__ dst, int C, int G, int r) {
   int b = blockIdx.z, g = blockIdx.y;

@@ -96,7 +96,11 @@ class PVCNN2Unet(nn.Module):
 
     @torch.no_grad()
     def forward_point_major(self, x, t=None, style=None, clip_feat=None, out=None):
-        """x [B,N,D] (D = 3 + extra) fp32 -> [B,N,num_classes]; the layout the kernels use."""
+        """x [B,N,D] (D = 3 + extra) fp32 -> [B,N,num_classes]; the layout the kernels use.
+
+        Inside torch.autocast("cuda", dtype=torch.float16) the second 3x3x3 convolution of every PVConv takes FP16
+        operands with fp32 accumulation (LION_FWD_CONV_FP16); everything else is computed as outside autocast, and the
+        output stays fp32 where the reference's autocast route returns fp16 (a deviation in favour of precision)."""
         B, N, D = x.shape
         assert D == self.in_channels
         m = L.model_for(self, L.KIND_UNET, self.lion_desc(), self.lion_params())
@@ -128,7 +132,8 @@ class PVCNN2Unet(nn.Module):
             if getattr(m, "style_key", None) != key:
                 L.check(L.lib().lion_unet_cache_style(m.h, L.ptr(style), L.ptr(clip_feat), B, L.stream()), "unet_cache_style")
                 m.style_key, m.style_ref = key, (style, clip_feat)
-            L.check(L.lib().lion_unet_forward(m.h, L.ptr(x), L.ptr(t), None, None, L.ptr(out), B, N, L.stream()), "unet_forward")
+            L.check(L.lib().lion_unet_forward_flags(m.h, L.ptr(x), L.ptr(t), None, None, L.ptr(out), B, N, L.forward_flags(),
+                                                    L.stream()), "unet_forward")
         return out
 
     def forward(self, inputs, **kwargs):

@@ -50,7 +50,12 @@ class Conv3d(nn.Conv3d):
     def forward(self, inputs, return_gn_stats=False):
         """inputs [B,Cin,r,r,r] -> [B,Cout,r,r,r]; with return_gn_stats also the per (shape, channel)
         sum and sum of squares over the voxels (float64 [B,Cout]) that the kernel's epilogue
-        accumulates for the AdaGN that follows."""
+        accumulates for the AdaGN that follows.
+
+        Inside torch.autocast("cuda", dtype=torch.float16) the shapes of a PVConv's second convolution
+        (Cin = Cout in {32, 64, 128}) run with FP16 operands (inputs and weights rounded to nearest even)
+        and fp32 accumulation; other shapes run as outside autocast.  The output stays fp32 (the
+        reference's cuDNN call returns fp16 there): a deviation in favour of precision."""
         B, C, r = inputs.shape[0], inputs.shape[1], inputs.shape[2]
         assert C == self.in_channels and inputs.dim() == 5 and inputs.shape[3] == r and inputs.shape[4] == r
         x = _f32c(inputs)
@@ -61,7 +66,8 @@ class Conv3d(nn.Conv3d):
             ssum = torch.empty(B, self.out_channels, device=x.device, dtype=torch.float64)
             ssq = torch.empty_like(ssum)
         with torch.cuda.device(x.device):
-            _run(L.lib().lion_conv3d_gn_fwd, m.h, L.ptr(x), L.ptr(out), L.ptr(ssum), L.ptr(ssq), B, L.stream())
+            _run(L.lib().lion_conv3d_gn_fwd_flags, m.h, L.ptr(x), L.ptr(out), L.ptr(ssum), L.ptr(ssq), B, L.forward_flags(),
+                 L.stream())
         return (out, ssum, ssq) if return_gn_stats else out
 
 

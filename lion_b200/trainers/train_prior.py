@@ -62,7 +62,8 @@ class Trainer(object):
         self.dae.eval()
         latent_shape = self.model.latent_shape()
         gen_x, nstep, ode_time, sample_time, output_fsample = self.fun_generate_samples_vada(
-            latent_shape, self.dae, self.diffusion_disc, self.model, num_shapes, enable_autocast=False, ode_sample=0,
+            latent_shape, self.dae, self.diffusion_disc, self.model, num_shapes, enable_autocast=self.cfg.sde.autocast_train,
+            ode_sample=0,
             need_denoise=self.cfg.eval.need_denoise, ddim_step=ddim_step, clip_feat=clip_feat)
         assert gen_x.shape[2] == self.cfg.ddpm.input_dim
         if gen_x.shape[1] > self.sample_num_points:

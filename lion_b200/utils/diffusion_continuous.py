@@ -36,7 +36,7 @@ class DiffusionBase(object):
                          condition_input=None, mixing_logit=None, use_cust_ode_func=0, init_t=1.0, return_all_sample=False,
                          clip_feat=None):
         """-> (samples [num_samples, *shape], nfe, seconds)  [+ all evaluated time points when return_all_sample]"""
-        assert not enable_autocast and not use_cust_ode_func, "lion_b200: fp32 / standard ODE function only"
+        assert not use_cust_ode_func, "lion_b200: standard ODE function only"
         assert not getattr(dae, 'mixed_prediction', False), "lion_b200: mixed_prediction is off in every shipped prior config"
         gc.collect()
         dae.eval()
@@ -52,9 +52,10 @@ class DiffusionBase(object):
             nfe[0] += 1
             if nfe[0] % 100 == 0:
                 logger.info('nfe_counter={}', nfe[0])
-            variance = self.var(t=t)
-            params = dae(x=x, t=t, condition_input=condition_input, clip_feat=clip_feat)
-            return self.f(t=t) * x + 0.5 * self.g2(t=t) * params / torch.sqrt(variance)
+            with torch.autocast("cuda", dtype=torch.float16, enabled=bool(enable_autocast)):
+                variance = self.var(t=t)
+                params = dae(x=x, t=t, condition_input=condition_input, clip_feat=clip_feat)
+                return self.f(t=t) * x + 0.5 * self.g2(t=t) * params / torch.sqrt(variance)
 
         # torchdiffeq's odeint integrates decreasing time spans by negating time: s = -t, dy/ds = -f(-s, y)
         def np_func(s, y):

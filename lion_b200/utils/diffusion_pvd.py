@@ -86,9 +86,11 @@ class DiffusionDiscretized(object):
     def run_denoising_diffusion(self, model, num_samples, shape, temp=1.0, enable_autocast=False, is_image=False,
                                 prior_var=1.0, condition_input=None, given_noise=None, clip_feat=None, cls_emb=None,
                                 grid_emb=None):
-        """Run the full denoising sampling loop (reference: diffusion_pvd.py:223-303)."""
-        if is_image or cls_emb is not None or grid_emb is not None or enable_autocast:
-            raise NotImplementedError("lion_b200: is_image / cls_emb / grid_emb / autocast are not used by LION's sampling path")
+        """Run the full denoising sampling loop (reference: diffusion_pvd.py:223-303).  enable_autocast runs the model
+        call under torch.autocast("cuda", float16) as the reference does, the captured step included (the mode is
+        baked into the graph); this package's networks return fp32 there."""
+        if is_image or cls_emb is not None or grid_emb is not None:
+            raise NotImplementedError("lion_b200: is_image / cls_emb / grid_emb are not used by LION's sampling path")
         if getattr(model, 'mixed_prediction', False):
             raise NotImplementedError("lion_b200: mixed prediction is disabled in every shipped prior config")
         model.eval()
@@ -131,7 +133,8 @@ class DiffusionDiscretized(object):
                 noise.copy_(given_noise[1][t].to(dev, torch.float32))
 
         def body(draw):
-            pred = model(x=x, t=tfl, condition_input=condition_input, clip_feat=clip_feat)
+            with torch.autocast("cuda", dtype=torch.float16, enabled=enable_autocast):
+                pred = model(x=x, t=tfl, condition_input=condition_input, clip_feat=clip_feat)
             if draw:
                 torch.randn(size, device=dev, out=noise)
             elif block is not None:
@@ -204,9 +207,10 @@ class DiffusionDiscretized(object):
         Noise: the reference draws `torch.randn(size)` on the CPU generator once per step and
         copies it to the device (:464-465); the S draws are made up front, in the same order,
         from the same generator (nothing else consumes it inside the loop), so a seeded run sees
-        the same values.  given_noise (extension, [S, *size]) replaces them."""
-        if grid_emb is not None or enable_autocast:
-            raise NotImplementedError("lion_b200: grid_emb / autocast are not used by LION's sampling path")
+        the same values.  given_noise (extension, [S, *size]) replaces them.  enable_autocast: as in
+        run_denoising_diffusion."""
+        if grid_emb is not None:
+            raise NotImplementedError("lion_b200: grid_emb is not used by LION's sampling path")
         if getattr(model, 'mixed_prediction', False):
             raise NotImplementedError("lion_b200: mixed prediction is disabled in every shipped prior config")
         model.eval()
@@ -237,7 +241,8 @@ class DiffusionDiscretized(object):
         lib = L.lib()
 
         def body():
-            pred = model(x=x, t=tfl, condition_input=condition_input, clip_feat=clip_feat)
+            with torch.autocast("cuda", dtype=torch.float16, enabled=enable_autocast):
+                pred = model(x=x, t=tfl, condition_input=condition_input, clip_feat=clip_feat)
             L.check(lib.lion_ddim_update(L.ptr(x), L.ptr(pred.contiguous()), L.ptr(noise), L.ptr(x), L.ptr(tables),
                                          L.ptr(step), n, L.ptr(hist), L.stream()), "ddim_update")
             L.check(lib.lion_ddim_next_step(L.ptr(step), L.ptr(tfl), L.ptr(tables), num_samples, S, L.stream()), "ddim_next_step")
