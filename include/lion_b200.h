@@ -199,6 +199,27 @@ int lion_pvconv_probe_flags(LionModel* m, const float* features, const float* co
 /* lion_attention_probe: a linear attention as lion_linear_attention_fwd runs it.  qkv [B, 3*heads*32, N] (q, k, v of
  * every head), o [B, heads*32, N] the output before the projection, out [B,C,N]. */
 int lion_attention_probe(LionModel* m, const float* x, float* qkv, float* o, float* out, int B, int N, void* stream);
+/* lion_fp_probe: an FP module as lion_fp_module_fwd runs it.  nn_idx / nn_wgt [B,3,N] the 3 nearest centres of every
+ * point and their weights; cat [B, cc + roundup(cp,4), N] the MLP input [interpolated | skip], padding channels
+ * included (NaN-filled before its producers run).  Per MLP layer l with C_l channels: raw / act [B,C_l,N] at offset
+ * B*N*(C_0 + ... + C_{l-1}) the raw 1x1 output and the activated output (the last layer's is the module output);
+ * gn_sum / gn_sqsum [B,C_l] (doubles) and the folded AdaGN scale / shift [B,C_l] at offset B*(C_0 + ... + C_{l-1}). */
+int lion_fp_probe(LionModel* m, const float* points_coords, const float* centers_coords, const float* centers_features,
+                  const float* points_features, const float* style, int* nn_idx, float* nn_wgt, float* cat, float* raw,
+                  float* act, double* gn_sum, double* gn_sqsum, float* scale, float* shift, int B, int N, int M, void* stream);
+/* lion_unet_probe: a U-Net forward as lion_unet_forward runs it (style == NULL: the lion_unet_cache_style vectors),
+ * with its glue copied into caller buffers as it is computed.  taps holds 4 + 6*n_fp + 5 device pointers, each may be
+ * NULL; PF = packed [B][ceil(C/4)][R][4]:
+ *   sinu, h, temb [B,E] (the sinusoid, after Linear + LeakyReLU, the time embedding); aff [B, style_total];
+ *   per FP stage: cf PF [C_in + E, M] (centre features after the time-embedding concat), nn_idx (int) and nn_wgt
+ *   [B][N][3], skip PF [roundup(cp,4), N], cat PF [cc + roundup(cp,4), N] (NaN-filled before its producers run),
+ *   out PF [C, N] (the stage's output after its PVConvs);
+ *   head: feat PF [C, N], cls_raw PF [128, N], cls_sums [2][B][128] (doubles), cls_aff [2][B][128] (scale, shift),
+ *   hc PF [128, N].
+ * style_table [n_style][2] (host, may be NULL): (offset, width) of every AdaGN style Linear's output in aff, in build
+ * order; n_style must be the network's number of them. */
+int lion_unet_probe(LionModel* m, const float* x, const float* t, const float* style, const float* clip, float* out,
+                    void* const* taps, int ntaps, int* style_table, int n_style, int B, int N, void* stream);
 /* Prior.forward with SE cells (models/score_sde/resnet.py:195-218): x [B,D], t [B], clip [B,clip_dim] or NULL */
 int lion_global_prior_forward(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                               void* stream);

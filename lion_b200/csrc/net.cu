@@ -270,8 +270,9 @@ int make_fp(Model* m, FPBlk& f, Cursor& cur, int cc, int cp, const std::vector<i
 struct PF { float4* p = nullptr; int G = 0; int R = 0; };
 struct VoxPrep { const float4* c4; int N, r; float4* nc; int* order; int* ppos; int* len; unsigned char* occ; int occ_stride;
                  int* cidx; int* nocc; int* vgrid; };   // compact ids of the occupied voxels (sparse first convolution) or null
-// Intermediate results of one SA module's MLP that lion_sa_mlp_probe copies out: device pointers into the forward's arena,
-// filled in by sa_fwd / shared_mlp_fwd when Fwd::rec is set (never in a product call).
+// Intermediate results of one MLP (an SA module's, an FP module's or the U-Net head's) that lion_sa_mlp_probe,
+// lion_fp_probe and lion_unet_probe copy out: device pointers into the forward's arena, filled in by sa_fwd / fp_fwd /
+// shared_mlp_fwd when Fwd::rec is set (never in a product call).
 constexpr int MLP_REC_MAX = 4;
 struct MlpRecord {
   int force = 0;                  // in: 0 = the path sa_fwd chooses, 1 = unfused kernels, 2 = fused (sa_fused.cu)
@@ -280,6 +281,22 @@ struct MlpRecord {
   const double* ssum[MLP_REC_MAX]; const double* ssq[MLP_REC_MAX]; int stat_stride[MLP_REC_MAX];
   const float* scale[MLP_REC_MAX]; const float* shift[MLP_REC_MAX];   // [B][C] folded AdaGN of each layer
   const float* pool_mm = nullptr; // last layer: [B][C/4][M][2][4] pre-activation minimum / maximum over the 32 neighbours
+  // unpooled layers: the raw 1x1 output (PF of C/4 groups) and the activated output, at act_off of act_G groups
+  const float4* raw[MLP_REC_MAX] = {}; const float4* act[MLP_REC_MAX] = {}; int act_G[MLP_REC_MAX] = {}, act_off[MLP_REC_MAX] = {};
+  const float4* cat = nullptr;    // FP module: the MLP input [interpolated | skip] (PF)
+};
+// Caller buffers (device) that lion_unet_probe has unet_forward fill.  The U-Net releases arena marks between stages,
+// so each result is copied out on the main stream where it is recorded, in the real pass only; a side-stream result
+// (3-NN, time embedding) only after the main stream's wait for its event.  PFs are copied in their packed layout
+// [B][G][R][4], the 3-NN in its [B][N][3] layout.  Any pointer may be null.
+constexpr int UNET_REC_FP = 8;
+struct UnetRecord {
+  float *sinu = nullptr, *h = nullptr, *temb = nullptr, *aff = nullptr;   // [B][E] x 3, [B][style_total]
+  struct Stage { float *cf, *nn_wgt, *skip, *cat, *out; int* nn_idx; } fp[UNET_REC_FP] = {};
+  float *feat = nullptr, *cls_raw = nullptr, *cls_aff = nullptr, *hc = nullptr;   // head; cls_aff [2][B][128]
+  double* cls_sums = nullptr;     // [2][B][128]
+  int stage = 0;                  // the FP stage running
+  const float *a_sinu = nullptr, *a_h = nullptr;                   // arena: the first two time-embedding stages
 };
 // Intermediate results of one PVConv (and its attention) that lion_pvconv_probe / lion_attention_probe copy out: device
 // pointers into the forward's arena, filled in by pvconv_fwd / attn_fwd when Fwd::pv is set (never in a product call).
@@ -301,15 +318,24 @@ struct Fwd {
   std::deque<VoxPrep> vox;       // a deque: get_vox hands out pointers that later preps must not move
   MlpRecord* rec = nullptr;      // test entry points only
   PvRecord* pv = nullptr;        // test entry points only
+  UnetRecord* ur = nullptr;      // test entry points only
   bool conv_f16 = false;         // LION_FWD_CONV_FP16: the PVConvs' second convolutions take FP16 operands (pvconv_fwd)
 };
-static void record_layer(Fwd& f, const AffSrc& a) {
+static bool record_layer(Fwd& f, const AffSrc& a) {
   MlpRecord* r = f.rec;
-  if (!r || r->n >= MLP_REC_MAX) return;
+  if (!r || r->n >= MLP_REC_MAX) return false;
   r->ssum[r->n] = a.ssum; r->ssq[r->n] = a.ssq; r->stat_stride[r->n] = a.stat_stride;
   r->scale[r->n] = a.scale; r->shift[r->n] = a.shift;
   r->n++;
+  return true;
 }
+// lion_unet_probe: copy `bytes` from the arena into a caller buffer now, on the main stream (real pass only)
+static int rec_copy(Fwd& f, void* dst, const void* src, size_t bytes) {
+  if (!dst || f.c->dry || !bytes) return 0;
+  LION_CHECK_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, f.c->stream));
+  return 0;
+}
+static size_t pf_bytes(const Fwd& f, const PF& p) { return sizeof(float4) * f.B * p.G * p.R; }
 // One point level of a forward: SA level i's input points, the centres its FPS samples from them (the points of
 // level i + 1) with their ball-query neighbours, and the 3-NN of the points among the centres that the FP stage
 // interpolating back onto them uses.  An event is set from the side stream's record of the result until the main
@@ -484,7 +510,8 @@ static int shared_mlp_fwd(Fwd& f, const SharedMLPBlk& m, PF in, int pool, float4
     }
     PF raw = alloc_pf(f, Gout, cur.R);
     LION_TRY(conv_gn(f, w, cur.p, cur.G, raw.p, Gout, geom_rows(cur.R), m.gn[i], (double)cur.R, nullptr, nullptr, a));
-    record_layer(f, a);
+    const int l = record_layer(f, a) ? f.rec->n - 1 : -1;
+    if (l >= 0) f.rec->raw[l] = raw.p;
     if (last && pool > 1) {
       if (pool != 32 || cur.R % 32) { set_error("shared_mlp: unsupported pooling %d", pool); return LION_ERR_ARG; }
       int Ro = cur.R / 32;
@@ -495,6 +522,7 @@ static int shared_mlp_fwd(Fwd& f, const SharedMLPBlk& m, PF in, int pool, float4
       if (last) { o = dst; gd = Gd; go = g_off; }
       else { nxt = alloc_pf(f, Gout, cur.R); o = nxt.p; gd = Gout; go = 0; }
       LION_LAUNCH(f.c, k_act_rows<1>, dim3(cdiv(cur.R, 256), Gout, f.B), 256, 0, raw.p, o, a, Gout, w.cout, cur.R, gd, go, last ? 0 : 1);
+      if (l >= 0) { f.rec->act[l] = o; f.rec->act_G[l] = gd; f.rec->act_off[l] = go; }
       cur = nxt;
     }
     LION_TRY(check_launch(f.c, "shared_mlp act"));
@@ -800,9 +828,19 @@ static int fp_fwd(Fwd& f, const FPBlk& b, Level& lv, PF cfeat, float4* dst, int 
   size_t mk = f.c->mark();
   LION_TRY(wait_once(f.c, lv.nn_done));
   PF cat = alloc_pf(f, Gc + Gs, N);
+  // probe mode: every float of cat a NaN first, so that a row or channel nobody writes shows up
+  if (f.rec || f.ur) LION_TRY(memset_async(f.c, cat.p, 0xff, pf_bytes(f, cat)));
   LION_LAUNCH(f.c, k_interp_rows, dim3(cdiv(N, 128), Gc, f.B), 128, 0, cfeat.p, lv.nn_idx, lv.nn_wgt, cat.p, Gc, M, N, Gc + Gs, 0);
   if (Gs) LION_LAUNCH(f.c, k_copy_groups, dim3(cdiv(N, 256), Gs, f.B), 256, 0, skip.p, cat.p, Gs, Gc + Gs, Gc, N);
   LION_TRY(check_launch(f.c, "fp interpolate"));
+  if (f.rec) f.rec->cat = cat.p;
+  if (f.ur) {
+    UnetRecord::Stage& s = f.ur->fp[f.ur->stage];
+    LION_TRY(rec_copy(f, s.nn_idx, lv.nn_idx, sizeof(int) * f.B * N * 3));
+    LION_TRY(rec_copy(f, s.nn_wgt, lv.nn_wgt, sizeof(float) * f.B * N * 3));
+    if (Gs) LION_TRY(rec_copy(f, s.skip, skip.p, pf_bytes(f, skip)));
+    LION_TRY(rec_copy(f, s.cat, cat.p, pf_bytes(f, cat)));
+  }
   LION_TRY(shared_mlp_fwd(f, b.mlp, cat, 1, dst, Gd, g_off));
   f.c->release(mk);
   return 0;
@@ -1051,6 +1089,7 @@ static int unet_side_stream(Fwd& f, const float* t, float* temb, std::vector<Lev
       // three tiny dependent launches (~45 us of latency) that nothing needs before level 1
       float* sinu = c->alloc_n<float>((size_t)B * E);
       float* h = c->alloc_n<float>((size_t)B * E);
+      if (f.ur) { f.ur->a_sinu = sinu; f.ur->a_h = h; }
       LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, sinu, E / 2, 1.0f);
       LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e0w, u.e0b, sinu, E, h, E, E, E, 1);
       LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e2w, u.e2b, h, E, temb, E, E, E, 0);
@@ -1096,6 +1135,7 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
     if (!f.m->aff_cache || f.m->aff_cache_B != B) { set_error("unet: no cached style for B=%d (call lion_unet_cache_style first)", B); return LION_ERR_STATE; }
     f.aff = f.m->aff_cache;
   }
+  if (f.ur) LION_TRY(rec_copy(f, f.ur->aff, f.aff, sizeof(float) * B * f.m->style_total));
   LION_TRY(check_launch(c, "unet prologue"));
   LION_TRY(stat_pool_begin(f, (size_t)f.m->style_total * f.B * sizeof(double) + 4096));   // sum(2*C) doubles per shape
 
@@ -1146,10 +1186,12 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
   }
   for (size_t j = 0; j < u.fp.size(); ++j) {
     Level& lv = L[n_sa - 1 - j];
+    if (f.ur) f.ur->stage = (int)j;
     for (auto& blk : u.fp[j]) {
       if (blk.kind == LION_KIND_FP) {
         PF cf = feat;
         if (temb) LION_TRY(with_temb(feat, &cf));          // torch.cat([features, temb]) (:160)
+        if (f.ur) LION_TRY(rec_copy(f, f.ur->fp[j].cf, cf.p, pf_bytes(f, cf)));
         PF o = alloc_pf(f, blk.fp.mlp.cout() / 4, lv.n);
         LION_TRY(fp_fwd(f, blk.fp, lv, cf, o.p, o.G, 0));
         feat = o;
@@ -1161,9 +1203,32 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
         stamp(c, c->stream, "fp.pvconv", (int)j);
       }
     }
+    if (f.ur) LION_TRY(rec_copy(f, f.ur->fp[j].out, feat.p, pf_bytes(f, feat)));
   }
   PF h = alloc_pf(f, 32, feat.R);
+  MlpRecord cls_rec;
+  if (f.ur) {
+    LION_TRY(rec_copy(f, f.ur->feat, feat.p, pf_bytes(f, feat)));
+    f.rec = &cls_rec;
+  }
   LION_TRY(shared_mlp_fwd(f, u.cls0, feat, 1, h.p, 32, 0));
+  if (f.ur) {
+    f.rec = nullptr;
+    UnetRecord& R = *f.ur;
+    const size_t BC = (size_t)B * 128;
+    LION_TRY(rec_copy(f, R.cls_raw, cls_rec.raw[0], pf_bytes(f, h)));
+    LION_TRY(rec_copy(f, R.hc, h.p, pf_bytes(f, h)));
+    if (R.cls_sums && !c->dry) {
+      LION_CHECK_CUDA(cudaMemcpy2DAsync(R.cls_sums, sizeof(double) * 128, cls_rec.ssum[0], sizeof(double) * cls_rec.stat_stride[0],
+                                        sizeof(double) * 128, B, cudaMemcpyDeviceToDevice, c->stream));
+      LION_CHECK_CUDA(cudaMemcpy2DAsync(R.cls_sums + BC, sizeof(double) * 128, cls_rec.ssq[0], sizeof(double) * cls_rec.stat_stride[0],
+                                        sizeof(double) * 128, B, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    if (R.cls_aff) {
+      LION_TRY(rec_copy(f, R.cls_aff, cls_rec.scale[0], sizeof(float) * BC));
+      LION_TRY(rec_copy(f, R.cls_aff + BC, cls_rec.shift[0], sizeof(float) * BC));
+    }
+  }
   if (u.num_classes == 4) {
     LION_TRY(run_conv(f, u.cls2, h.p, h.G, (float4*)out, 1, nullptr, nullptr, geom_rows(feat.R)));
   } else {
@@ -1173,6 +1238,11 @@ static int unet_forward(Fwd& f, const float* x, const float* t, const float* sty
   }
   // never consumed by a one-level network: still join the side stream (every other result was waited for above)
   LION_TRY(wait_once(c, temb_done));
+  if (f.ur && temb) {
+    LION_TRY(rec_copy(f, f.ur->sinu, f.ur->a_sinu, sizeof(float) * B * E));
+    LION_TRY(rec_copy(f, f.ur->h, f.ur->a_h, sizeof(float) * B * E));
+    LION_TRY(rec_copy(f, f.ur->temb, temb, sizeof(float) * B * E));
+  }
   stamp(c, c->stream, "end");
   return check_launch(c, "unet epilogue");
 }
@@ -1755,6 +1825,104 @@ extern "C" int lion_attention_probe(LionModel* h, const float* x, float* qkv, fl
     from_pf(f, y, out, a.C);
     return check_launch(f.c, "lion_attention_probe");
   });
+}
+
+// [B][N][3] 32-bit words -> [B][3][N]: the 3-NN indices or weights in the reference's layout
+__global__ void k_nn_to_cm(const unsigned* __restrict__ src, unsigned* __restrict__ dst, int N) {
+  int b = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  for (int k = 0; k < 3; ++k) dst[((size_t)b * 3 + k) * N + j] = src[((size_t)b * N + j) * 3 + k];
+}
+
+// An FP module as lion_fp_module_fwd runs it: nn_idx / nn_wgt [B,3,N] the 3-NN; cat [B, cc + roundup(cp,4), N] the MLP
+// input, padding channels included (NaN-filled before its producers run); per layer l (C_l channels): raw / act
+// [B,C_l,N] at offset B N (C_0 + ... + C_{l-1}) the raw 1x1 output and the activated output (the last is the module
+// output), gn_sum / gn_sqsum (doubles) and the folded scale / shift [B,C_l] at offset B (C_0 + ... + C_{l-1}).
+extern "C" int lion_fp_probe(LionModel* h, const float* points_coords, const float* centers_coords, const float* centers_features,
+                             const float* points_features, const float* style, int* nn_idx, float* nn_wgt, float* cat, float* raw,
+                             float* act, double* gn_sum, double* gn_sqsum, float* scale, float* shift, int B, int N, int M,
+                             void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_FP, "lion_fp_probe: not an FP model");
+  LION_REQUIRE(points_coords && centers_coords && centers_features && style && nn_idx && nn_wgt && cat && raw && act && gn_sum &&
+               gn_sqsum && scale && shift && B > 0 && N > 0 && M > 0, "lion_fp_probe: bad arguments");
+  Model* m = &h->m;
+  const FPBlk& b = m->block->fp;
+  LION_REQUIRE((b.cp > 0) == (points_features != nullptr), "lion_fp_probe: points_features presence does not match the module");
+  LION_REQUIRE((int)b.mlp.conv.size() <= MLP_REC_MAX, "lion_fp_probe: more than %d layers", MLP_REC_MAX);
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    MlpRecord rec;
+    f.rec = &rec;
+    LION_TRY(style_affine_all(f, style));
+    Level lv{to_c4(f, points_coords, N), N};
+    lv.centers = to_c4(f, centers_coords, M); lv.m = M;
+    PF cf = to_pf(f, centers_features, b.cc, M);
+    if (b.cp) lv.feat = to_pf(f, points_features, b.cp, N);
+    PF o = alloc_pf(f, b.mlp.cout() / 4, N);
+    LION_TRY(fp_geometry(f, f.c->stream, lv, 0));
+    LION_TRY(fp_fwd(f, b, lv, cf, o.p, o.G, 0));
+    // (the arena fp_fwd released is not reused before these copies: they are the next work on the stream)
+    LION_LAUNCH(f.c, k_nn_to_cm, dim3(cdiv(N, 256), B), 256, 0, (const unsigned*)lv.nn_idx, (unsigned*)nn_idx, N);
+    LION_LAUNCH(f.c, k_nn_to_cm, dim3(cdiv(N, 256), B), 256, 0, (const unsigned*)lv.nn_wgt, (unsigned*)nn_wgt, N);
+    const int Gcat = b.mlp.cin_pad / 4;
+    LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), Gcat, B), 256, 0, rec.cat, cat, 4 * Gcat, Gcat, N);
+    size_t off = 0;
+    for (int l = 0; l < (int)b.mlp.conv.size(); ++l) {
+      const int C = b.mlp.conv[l].cout, G = C / 4;
+      if (l >= rec.n || !rec.raw[l] || !rec.act[l] || rec.act_G[l] != G || rec.act_off[l] != 0) {
+        set_error("lion_fp_probe: layer %d was not recorded", l);
+        return LION_ERR_STATE;
+      }
+      LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.raw[l], raw + off * N, C, G, N);
+      LION_LAUNCH(f.c, k_pf_to_cm, dim3(cdiv(N, 256), G, B), 256, 0, rec.act[l], act + off * N, C, G, N);
+      if (!f.c->dry) {
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sum + off, sizeof(double) * C, rec.ssum[l], sizeof(double) * rec.stat_stride[l],
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sqsum + off, sizeof(double) * C, rec.ssq[l], sizeof(double) * rec.stat_stride[l],
+                                          sizeof(double) * C, B, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpyAsync(scale + off, rec.scale[l], sizeof(float) * B * C, cudaMemcpyDeviceToDevice, f.c->stream));
+        LION_CHECK_CUDA(cudaMemcpyAsync(shift + off, rec.shift[l], sizeof(float) * B * C, cudaMemcpyDeviceToDevice, f.c->stream));
+      }
+      off += (size_t)B * C;
+    }
+    return check_launch(f.c, "lion_fp_probe");
+  });
+}
+
+// A U-Net forward as lion_unet_forward runs it, with its glue recorded.  taps: 4 + 6 n_fp + 5 device pointers, any of
+// them NULL (not recorded), in this order (PF = packed [B][G][R][4], G = ceil(C / 4)):
+//   sinu, h, temb [B][E]: the sinusoid, after the first Linear + LeakyReLU, the time embedding;
+//   aff [B][style_total]: every AdaGN (factor | bias) vector, as computed (style != NULL) or cached (style == NULL);
+//   per FP stage j: cf PF [C_in + E, M] the centre features after the time-embedding concat; nn_idx (int) / nn_wgt
+//   [B][N][3] the 3-NN of the level's points; skip PF [roundup(cp,4), N] the level's skip features (not written when
+//   cp = 0); cat PF [cc + roundup(cp,4), N] the MLP input (NaN-filled before its producers run); out PF [C_j, N] the
+//   stage's output after its PVConvs;
+//   head: feat PF [C, N] its input; cls_raw PF [128, N] cls0's raw output; cls_sums [2][B][128] (doubles) its
+//   GroupNorm sums; cls_aff [2][B][128] its folded scale / shift; hc PF [128, N] its output.
+// style_table [n_style][2] (host): (out_off, n_out) of every AdaGN style Linear in build order.
+extern "C" int lion_unet_probe(LionModel* h, const float* x, const float* t, const float* style, const float* clip, float* out,
+                               void* const* taps, int ntaps, int* style_table, int n_style, int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_UNET, "lion_unet_probe: not a unet model");
+  LION_REQUIRE(x && out && taps && B > 0 && N > 0, "lion_unet_probe: bad arguments");
+  Model* m = &h->m;
+  const int n_fp = (int)m->unet->fp.size();
+  LION_REQUIRE(n_fp <= UNET_REC_FP, "lion_unet_probe: more than %d FP stages", UNET_REC_FP);
+  LION_REQUIRE(ntaps == 4 + 6 * n_fp + 5, "lion_unet_probe: %d taps given, %d expected", ntaps, 4 + 6 * n_fp + 5);
+  LION_REQUIRE(n_style == (int)m->style_layers.size(), "lion_unet_probe: %d style layers expected, the network has %d", n_style,
+               (int)m->style_layers.size());
+  for (int i = 0; style_table && i < n_style; ++i) {
+    style_table[2 * i] = m->style_layers[i].out_off;
+    style_table[2 * i + 1] = m->style_layers[i].n_out;
+  }
+  UnetRecord rec;
+  int k = 0;
+  auto tap = [&]() { return (float*)taps[k++]; };
+  rec.sinu = tap(); rec.h = tap(); rec.temb = tap(); rec.aff = tap();
+  for (int j = 0; j < n_fp; ++j) {
+    UnetRecord::Stage& s = rec.fp[j];
+    s.cf = tap(); s.nn_idx = (int*)tap(); s.nn_wgt = tap(); s.skip = tap(); s.cat = tap(); s.out = tap();
+  }
+  rec.feat = tap(); rec.cls_raw = tap(); rec.cls_sums = (double*)tap(); rec.cls_aff = tap(); rec.hc = tap();
+  return two_pass(m, stream, B, [&](Fwd& f) { f.ur = &rec; return unet_forward(f, x, t, style, clip, out, N); });
 }
 
 extern "C" int lion_global_prior_step(LionModel* h, const float* x, const float* t, const float* clip, float* out, int B,

@@ -337,7 +337,8 @@ def three_nn(points, centers):
 
     Brute-force 3 smallest squared distances with the kernel's strict '<' cascade (a later
     centre never displaces an equal earlier one), clamp to [1e-10,1e10], weights
-    d1d2/(d0d1+d0d2+d1d2) etc. (:61-73)."""
+    d1d2/(d0d1+d0d2+d1d2) etc. (:61-73).  With fewer than three centres the missing slots keep
+    the kernel's initial index 0 and distance 1e40 (:37-38), which the clamp turns into 1e10."""
     pt = _f32(torch.as_tensor(points).numpy())
     ce = _f32(torch.as_tensor(centers).numpy())
     B, _, N = pt.shape
@@ -349,10 +350,10 @@ def three_nn(points, centers):
                     pt[b, 1][:, None] - ce[b, 1][None, :],
                     pt[b, 2][:, None] - ce[b, 2][None, :])           # [N,M]
         order = np.argsort(d, axis=1, kind="stable")[:, :3]          # stable == strict '<' cascade
-        if M < 3:  # unreachable in LION (M >= 16); kernel would keep index 0 / 1e40
-            pad = np.zeros((N, 3 - M), dtype=order.dtype)
-            order = np.concatenate([order, pad], axis=1)
         best = np.take_along_axis(d, order, axis=1).astype(np.float32)
+        if M < 3:  # unreachable in LION (M >= 16): the slots no centre filled keep index 0 and 1e40
+            order = np.concatenate([order, np.zeros((N, 3 - M), dtype=order.dtype)], axis=1)
+            best = np.concatenate([best, np.full((N, 3 - M), np.inf, dtype=np.float32)], axis=1)
         best = np.maximum(np.minimum(np.float32(1e10), best), np.float32(1e-10))
         d0, d1, d2 = best[:, 0], best[:, 1], best[:, 2]
         d0d1 = (d0 * d1).astype(np.float32)

@@ -271,3 +271,46 @@ def attn_out(o, wo, bo, tc=True):
     rna, trunc = operand_models(tc)
     w = rna(wo.reshape(wo.shape[0], -1).contiguous()).double()
     return torch.einsum("oc,bcn->bon", w, trunc(o).double()) + bo.double()[None, :, None]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# FP module: 3-NN interpolation, [interpolated | skip] concatenation, unpooled MLP; the U-Net's glue
+# ---------------------------------------------------------------------------------------------------------------------
+def interp_fma(cf, idx, wgt):
+    """k_interp_rows in fp32: f0 * w0, then fma(f1, w1, .), then fma(f2, w2, .).  cf [B,C,M] fp32, idx [B,3,N], wgt
+    [B,3,N] fp32 -> [B,C,N] fp32 (each fma through float64, where a * b is exact)."""
+    B, C, _ = cf.shape
+    N = idx.shape[-1]
+    g = [cf.gather(2, idx[:, k].long()[:, None, :].expand(B, C, N)).double() for k in range(3)]
+    w = [wgt[:, k][:, None, :].double() for k in range(3)]
+    a = (g[0] * w[0]).float()
+    a = (g[1] * w[1] + a.double()).float()
+    return (g[2] * w[2] + a.double()).float()
+
+
+def act_rows(raw, scale, shift, rna):
+    """k_act_rows<1>: swish(fma(raw, scale, shift)), rounded to TF32 (rna) where the next layer reads it.
+    raw fp32 [B,C,N], scale / shift fp32 [B,C] -> fp32 [B,C,N] (the swish in float64)."""
+    a = (raw.double() * scale[:, :, None].double() + shift[:, :, None].double()).float().double()
+    y = (a * torch.sigmoid(a)).float()
+    return tf32_rna(y) if rna else y
+
+
+def mlp_fold(sums, sqs, sd, p, style, count):
+    """fold_affine of the AdaGN at state-dict prefix p (norm.*, emd.*) from per-channel sums."""
+    fb = style.double() @ sd[p + "emd.weight"].double().T + sd[p + "emd.bias"].double()
+    return fold_affine(sums, sqs, sd[p + "norm.weight"].double(), sd[p + "norm.bias"].double(), fb, count)
+
+
+def sinusoid(t, E):
+    """k_time_sinusoid in float64 of the kernel's fp32 argument e = fl(t * freq), freq = fl(exp(float64)) as build_unet
+    computes it.  t fp32 [B] -> float64 [B, E] (sin | cos)."""
+    half = E // 2
+    fr = torch.from_numpy(np.exp(np.arange(half, dtype=np.float64) * -(np.log(10000.0) / (half - 1))).astype(np.float32))
+    e = (t.float()[:, None].cpu() * fr[None, :]).double()
+    return torch.cat([torch.sin(e), torch.cos(e)], 1)
+
+
+def linear_f64(x, w, b, leaky=False):
+    y = x.double() @ w.double().T + b.double()
+    return torch.where(y > 0, y, 0.1 * y) if leaky else y

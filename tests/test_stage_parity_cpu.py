@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import point_ops as OP
 from tests import stage_ref as SR
 
 
@@ -166,3 +167,107 @@ def test_act_grid_model_matches_its_definition():
                 y = np.float32(np.float64(a) / (1.0 + np.exp(-np.float64(a))))
                 want = _tf32_bits_reference(torch.tensor([y]), "rna")[0].item()
                 assert inner[b, c].flatten()[i].item() == want
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# FP module and the U-Net's glue (tests/test_fp_stage_gpu.py, test_unet_glue_stage_gpu.py)
+# ---------------------------------------------------------------------------------------------------------------------
+def _three_nn_scalar(pt, ce):
+    """neighbor_interpolate.cu:36-73 transcribed literally for one shape: double best distances starting at 1e40, the
+    strict '<' cascade, the clamp to [1e-10, 1e10] in double, products rounded to float, fp32 sum and reciprocal."""
+    f32 = np.float32
+    N, M = pt.shape[1], ce.shape[1]
+    idx, wgt = np.zeros((3, N), np.int32), np.zeros((3, N), np.float32)
+    for j in range(N):
+        best, bi = [1e40, 1e40, 1e40], [0, 0, 0]
+        for k in range(M):
+            dx, dy, dz = (f32(pt[a, j]) - f32(ce[a, k]) for a in range(3))
+            d = float(OP._sqdist(dx, dy, dz))
+            if d < best[2]:
+                best[2], bi[2] = d, k
+                if d < best[1]:
+                    best[2], bi[2], best[1], bi[1] = best[1], bi[1], d, k
+                    if d < best[0]:
+                        best[1], bi[1], best[0], bi[0] = best[0], bi[0], d, k
+        b = [max(min(float(f32(1e10)), v), float(f32(1e-10))) for v in best]
+        d0d1, d0d2, d1d2 = f32(b[0] * b[1]), f32(b[0] * b[2]), f32(b[1] * b[2])
+        inv = f32(f32(1.0) / f32(f32(d0d1 + d0d2) + d1d2))
+        wgt[:, j] = [f32(d1d2 * inv), f32(d0d2 * inv), f32(d0d1 * inv)]
+        idx[:, j] = bi
+    return idx, wgt
+
+
+@pytest.mark.parametrize("M,kind", [(1, "gauss"), (2, "gauss"), (3, "gauss"), (40, "gauss"), (30, "ties"), (20, "dup")])
+def test_three_nn_oracle_matches_the_reference_cascade(M, kind):
+    """The oracle's 3-NN against a scalar transcription of the reference kernel, including fewer than three centres
+    (the missing slots keep index 0 and distance 1e40) and exact distance ties (the lower index stays first)."""
+    g = torch.Generator().manual_seed(M)
+    if kind == "ties":
+        pts = torch.randint(-4, 4, (2, 3, 60), generator=g).float() / 4
+        ce = torch.randint(-2, 2, (2, 3, M), generator=g).float() / 2
+    else:
+        pts, ce = torch.randn(2, 3, 60, generator=g) * 0.3, torch.randn(2, 3, M, generator=g) * 0.3
+        if kind == "dup":
+            ce = torch.cat([ce[:, :, :M // 2]] * 2, 2)
+    idx, wgt = OP.three_nn(pts, ce)
+    for b in range(2):
+        ri, rw = _three_nn_scalar(pts[b].numpy(), ce[b].numpy())
+        assert np.array_equal(idx[b].numpy(), ri) and np.array_equal(wgt[b].numpy(), rw)
+    if M < 3:                                             # a missing slot (distance clamped to 1e10) weighs next to nothing
+        assert (idx[:, M:] == 0).all() and (wgt[:, M:] < 1e-9).all()
+
+
+def test_fp_references_restate_the_oracle():
+    from lion_b200.models.pvcnn2_ada import PointNetFPModule
+    from oracle import net as ON
+    from oracle import point_ops as OP
+    cc, cp, outs, N, M, B = 24, 5, [32, 16], 90, 20, 2
+    sd = _sd(PointNetFPModule(cc + cp, outs, cfg=_cfg()), 10)
+    g = torch.Generator().manual_seed(11)
+    pc, ce = torch.randn(B, 3, N, generator=g) * 0.3, torch.randn(B, 3, M, generator=g) * 0.3
+    cf, pf, style = torch.randn(B, cc, M, generator=g), torch.randn(B, cp, N, generator=g), torch.randn(B, 128, generator=g)
+    idx, wgt = OP.three_nn(pc, ce)
+    x = torch.cat([SR.interp_fma(cf, idx, wgt), pf], 1)
+    for l, c in enumerate(outs):
+        raw = SR.point_conv(x, sd["mlp.layers.%d.weight" % (3 * l)], sd["mlp.layers.%d.bias" % (3 * l)], tc=False)
+        s, t = SR.mlp_fold(raw.sum(2), (raw * raw).sum(2), sd, "mlp.layers.%d." % (3 * l + 1), style, float(N))
+        x = SR.act_rows(raw.float(), s.float(), t.float(), rna=False)
+    ref, _ = ON.fp_module(sd, "", dict(kind="fp", cin=cc + cp, mlp=outs), pc, ce, cf, pf, None, style)
+    assert _rel(x, ref) < 2e-5
+    # the interpolation is the oracle's up to the fused multiply-adds
+    assert _rel(SR.interp_fma(cf, idx, wgt), OP.nearest_neighbor_interpolate(pc, ce, cf)) < 1e-6
+
+
+def test_time_embedding_reference_restates_the_oracle():
+    import torch.nn.functional as TF
+    from oracle import net as ON
+    E = 64
+    t = torch.tensor([0.0, 1.0, 500.0, 999.0, 1000.0])
+    sinu = SR.sinusoid(t, E)
+    assert (sinu - ON.timestep_embedding(t, E).double()).abs().max() < 2e-6
+    g = torch.Generator().manual_seed(12)
+    w0, b0, w2, b2 = (torch.randn(E, E, generator=g) * 0.2, torch.randn(E, generator=g) * 0.1,
+                      torch.randn(E, E, generator=g) * 0.2, torch.randn(E, generator=g) * 0.1)
+    got = SR.linear_f64(SR.linear_f64(sinu, w0, b0, leaky=True), w2, b2)
+    ref = TF.linear(TF.leaky_relu(TF.linear(ON.timestep_embedding(t, E), w0, b0), 0.1), w2, b2)
+    assert _rel(got, ref) < 1e-5
+
+
+def test_classifier_reference_restates_the_oracle():
+    from oracle import net as ON
+    from tests.synth import synth_state_dict
+    C, N, B, nc = 64, 80, 2, 3
+    shapes = {"classifier.0.layers.0.weight": [128, C, 1], "classifier.0.layers.0.bias": [128],
+              "classifier.0.layers.1.norm.weight": [128], "classifier.0.layers.1.norm.bias": [128],
+              "classifier.0.layers.1.emd.weight": [256, 128], "classifier.0.layers.1.emd.bias": [256],
+              "classifier.2.weight": [nc, 128, 1], "classifier.2.bias": [nc]}
+    sd = synth_state_dict(shapes, 13)
+    g = torch.Generator().manual_seed(14)
+    feat, style = torch.randn(B, C, N, generator=g), torch.randn(B, 128, generator=g)
+    raw = SR.point_conv(feat, sd["classifier.0.layers.0.weight"], sd["classifier.0.layers.0.bias"], tc=False)
+    s, t = SR.mlp_fold(raw.sum(2), (raw * raw).sum(2), sd, "classifier.0.layers.1.", style, float(N))
+    hc = SR.act_rows(raw.float(), s.float(), t.float(), rna=False)
+    out = torch.einsum("oc,bcn->bon", sd["classifier.2.weight"].reshape(nc, 128).double(), hc.double()) + sd["classifier.2.bias"].double()[None, :, None]
+    h = ON.shared_mlp(sd, "classifier.0.", feat, style, 1)
+    ref = torch.einsum("oc,bcn->bon", sd["classifier.2.weight"].reshape(nc, 128), h) + sd["classifier.2.bias"][None, :, None]
+    assert _rel(out, ref) < 2e-5
