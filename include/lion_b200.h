@@ -223,6 +223,13 @@ int lion_unet_probe(LionModel* m, const float* x, const float* t, const float* s
 /* Prior.forward with SE cells (models/score_sde/resnet.py:195-218): x [B,D], t [B], clip [B,clip_dim] or NULL */
 int lion_global_prior_forward(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                               void* stream);
+/* lion_global_prior_probe: a global-prior forward as lion_global_prior_forward runs it, with every Linear's output
+ * copied into caller buffers.  taps holds 5 + 4*ncell device pointers [B, width] fp32, each may be NULL:
+ *   pe [emb] (the positional embedding), t0 [4*emb] (first temb Linear), temb [nf] (second temb Linear),
+ *   cmap [nf] (clip_feat_mapping; CLIP networks only, NULL otherwise), h0 [nf] (input layer);
+ *   per cell: a [nf] (conv1 + ReLU), bb [nf] (conv2 + ReLU), s [nf/8] (SE fc0 + ReLU), h [nf] (sigmoid(fc2) * bb + h). */
+int lion_global_prior_probe(LionModel* m, const float* x, const float* t, const float* clip, float* out,
+                            void* const* taps, int ntaps, int B, void* stream);
 /* the same call under the name SURVEY.md 8(b) lists (one denoising-step evaluation of the global prior) */
 int lion_global_prior_step(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                            void* stream);

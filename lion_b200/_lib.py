@@ -80,6 +80,7 @@ def _proto(lib):
         "lion_fp_probe": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_unet_probe": (P(vp, vp, vp, vp, vp, vp, C.POINTER(vp), i, C.POINTER(i), i, i, i, vp), i),
         "lion_global_prior_step": (P(vp, vp, vp, vp, vp, i, vp), i),
+        "lion_global_prior_probe": (P(vp, vp, vp, vp, vp, C.POINTER(vp), i, i, vp), i),
         "lion_workspace_bytes": (P(vp), sz),
         "lion_ddim_update": (P(vp, vp, vp, vp, vp, vp, sz, vp, vp), i),
         "lion_ddim_set_step": (P(vp, vp, vp, i, i, i, vp), i),

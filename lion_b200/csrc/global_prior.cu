@@ -177,11 +177,12 @@ __global__ void k_gp_reduce(const float* __restrict__ part, int nsplit, const fl
 // PositionalEmbedding (models/utils.py:16-31): fp32 frequencies exp(i * -log(1e4)/(half-1))
 __global__ void k_gp_posemb(const float* __restrict__ t, const float* __restrict__ freqs, float* __restrict__ out,
                             int half, float scale) {
-  int b = blockIdx.x, i = threadIdx.x;
-  if (i >= half) return;
-  float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);
-  out[(size_t)b * 2 * half + i] = sinf(e);
-  out[(size_t)b * 2 * half + half + i] = cosf(e);
+  const int b = blockIdx.x;
+  for (int i = threadIdx.x; i < half; i += blockDim.x) {     // any embedding_dim, whatever the block size
+    float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);
+    out[(size_t)b * 2 * half + i] = sinf(e);
+    out[(size_t)b * 2 * half + half + i] = cosf(e);
+  }
 }
 
 struct GPLin { const float* w; const float* b; int K, O; };
@@ -230,9 +231,12 @@ int global_prior_build(Model* m, Cursor& cur) {
 
 static int gp_linear(Ctx* c, const GPLin& l, const float* x, int xs, const float* add, int as, float* out, int os,
                      const float* mul, int ms, const float* res, int rs, int B, int act) {
-  if (l.K % 4) { set_error("global prior: K=%d must be a multiple of 4", l.K); return LION_ERR_ARG; }
+  if (l.K % 4) { set_error("global prior: K=%d must be a multiple of 4 (16-byte loads)", l.K); return LION_ERR_ARG; }
   int nsplit = cdiv(l.K, GP_KS);
-  if (nsplit > GP_MAXSPLIT) { set_error("global prior: K=%d too large", l.K); return LION_ERR_ARG; }
+  if (nsplit > GP_MAXSPLIT) {
+    set_error("global prior: K=%d needs %d K slices of %d, at most %d (K <= %d)", l.K, nsplit, GP_KS, GP_MAXSPLIT, GP_KS * GP_MAXSPLIT);
+    return LION_ERR_ARG;
+  }
   const size_t smem = (size_t)(GP_OB + GP_BT) * GP_PITCH * sizeof(float);
   static DevOnce attr_once;
   if (attr_once.need()) LION_CHECK_CUDA(cudaFuncSetAttribute(k_gp_partial, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -245,8 +249,18 @@ static int gp_linear(Ctx* c, const GPLin& l, const float* x, int xs, const float
   return 0;
 }
 
-// one chunk of <= 32 shapes: two kernels per Linear (split-K partial sums + deterministic reduce with fused epilogue)
-static int global_prior_forward_layers(Model* m, const float* x, const float* t, const float* clip, float* out, int B) {
+// lion_global_prior_probe: rows [b0, b0 + B) of a [.][w] caller buffer from `src` (row stride ss), real pass only
+static int gp_tap(Ctx* c, float* dst, int b0, const float* src, int ss, int w, int B) {
+  if (!dst || c->dry) return 0;
+  LION_CHECK_CUDA(cudaMemcpy2DAsync(dst + (size_t)b0 * w, w * sizeof(float), src, ss * sizeof(float), w * sizeof(float), B,
+                                    cudaMemcpyDeviceToDevice, c->stream));
+  return 0;
+}
+
+// one chunk of <= 32 shapes (rows b0 .. b0 + B - 1 of the call): two kernels per Linear (split-K partial sums +
+// deterministic reduce with fused epilogue)
+static int global_prior_forward_layers(Model* m, const float* x, const float* t, const float* clip, float* out, int B,
+                                       const GpRecord* rec, int b0) {
   GlobalPriorBlk* g = m->gp;
   Ctx* c = m->ctx;
   int nf = g->nf, tw = g->clip ? 2 * nf : nf;
@@ -259,16 +273,27 @@ static int global_prior_forward_layers(Model* m, const float* x, const float* t,
   float* a = c->alloc_n<float>((size_t)B * nf);
   float* bb = c->alloc_n<float>((size_t)B * nf);
   float* s0 = c->alloc_n<float>((size_t)B * nf / 8);
+  const GpRecord no_rec;
+  const GpRecord& r = rec ? *rec : no_rec;
   LION_LAUNCH(c, k_gp_posemb, B, 64, 0, t, g->d_freqs, pe, g->emb / 2, g->scale);
+  LION_TRY(gp_tap(c, r.pe, b0, pe, g->emb, g->emb, B));
   // temb_layer: two 1x1 convs, no nonlinearity in between (resnet.py:181-184)
   LION_TRY(gp_linear(c, g->t0, pe, g->emb, nullptr, 0, t0, g->emb * 4, nullptr, 0, nullptr, 0, B, 0));
+  LION_TRY(gp_tap(c, r.t0, b0, t0, g->emb * 4, g->emb * 4, B));
   if (g->clip) LION_TRY(memset_async(c, tadd, 0, sizeof(float) * B * tw));
   LION_TRY(gp_linear(c, g->t1, t0, g->emb * 4, nullptr, 0, tadd, tw, nullptr, 0, nullptr, 0, B, 0));
+  LION_TRY(gp_tap(c, r.temb, b0, tadd, tw, nf, B));
   // clip_feat_mapping output is concatenated behind temb (resnet.py:203-208) and reaches every
   // cell's conv1 un-added (ResBlockSEClip.forward, resnet.py:41-46)
-  if (g->clip) LION_TRY(gp_linear(c, g->cmap, clip, g->clip_dim, nullptr, 0, cat + nf, tw, nullptr, 0, nullptr, 0, B, 0));
+  if (g->clip) {
+    LION_TRY(gp_linear(c, g->cmap, clip, g->clip_dim, nullptr, 0, cat + nf, tw, nullptr, 0, nullptr, 0, B, 0));
+    LION_TRY(gp_tap(c, r.cmap, b0, cat + nf, tw, nf, B));
+  }
   LION_TRY(gp_linear(c, g->in, x, g->D, nullptr, 0, h, nf, nullptr, 0, nullptr, 0, B, 0));
-  for (auto& cell : g->cells) {
+  LION_TRY(gp_tap(c, r.h0, b0, h, nf, nf, B));
+  for (size_t k = 0; k < g->cells.size(); ++k) {
+    const auto& cell = g->cells[k];
+    const GpRecord::Cell rc = r.cells ? r.cells[k] : GpRecord::Cell{};
     // conv1(x + t [| clip]) -> ReLU -> (dropout: identity in eval) -> conv2 -> ReLU -> SE -> + x
     if (g->clip) {
       if (!c->dry)
@@ -277,16 +302,20 @@ static int global_prior_forward_layers(Model* m, const float* x, const float* t,
     } else {
       LION_TRY(gp_linear(c, cell.c1, h, nf, tadd, tw, a, nf, nullptr, 0, nullptr, 0, B, 1));
     }
+    LION_TRY(gp_tap(c, rc.a, b0, a, nf, nf, B));
     LION_TRY(gp_linear(c, cell.c2, a, nf, nullptr, 0, bb, nf, nullptr, 0, nullptr, 0, B, 1));
+    LION_TRY(gp_tap(c, rc.bb, b0, bb, nf, nf, B));
     LION_TRY(gp_linear(c, cell.se0, bb, nf, nullptr, 0, s0, nf / 8, nullptr, 0, nullptr, 0, B, 1));
+    LION_TRY(gp_tap(c, rc.s, b0, s0, nf / 8, nf / 8, B));
     LION_TRY(gp_linear(c, cell.se2, s0, nf / 8, nullptr, 0, h2, nf, bb, nf, h, nf, B, 2));   // sigmoid(.) * bb + h
+    LION_TRY(gp_tap(c, rc.h, b0, h2, nf, nf, B));
     float* tmp = h; h = h2; h2 = tmp;
   }
   LION_TRY(gp_linear(c, g->outl, h, nf, nullptr, 0, out, g->D, nullptr, 0, nullptr, 0, B, 0));
   return check_launch(c, "global_prior_forward");
 }
 
-int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B) {
+int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B, const GpRecord* rec) {
   GlobalPriorBlk* g = m->gp;
   Ctx* c = m->ctx;
   if (g->clip && !clip) { set_error("global prior: this network needs clip_feat"); return LION_ERR_ARG; }
@@ -297,7 +326,7 @@ int global_prior_forward(Model* m, const float* x, const float* t, const float* 
     const float* xc = x + (size_t)b0 * g->D;
     const float* cc = clip ? clip + (size_t)b0 * g->clip_dim : nullptr;
     float* oc = out + (size_t)b0 * g->D;
-    LION_TRY(global_prior_forward_layers(m, xc, t + b0, cc, oc, nb));
+    LION_TRY(global_prior_forward_layers(m, xc, t + b0, cc, oc, nb, rec, b0));
     c->release(mk);
   }
   return 0;

@@ -102,8 +102,16 @@ struct StyleEncBlk {
   const float* mlp_w = nullptr; const float* mlp_b = nullptr;
 };
 struct GlobalPriorBlk;   // global_prior.cu
+// Caller buffers (device, [B][width] fp32) that lion_global_prior_probe has global_prior_forward fill, each copied on
+// the stream right after the Linear that produced it (real pass only; never set in a product call).  Any may be null.
+struct GpRecord {
+  float *pe = nullptr, *t0 = nullptr, *temb = nullptr, *cmap = nullptr, *h0 = nullptr;   // [emb], [4 emb], [nf] x 3
+  struct Cell { float *a, *bb, *s, *h; };   // conv1 + ReLU, conv2 + ReLU [nf]; SE fc0 + ReLU [nf/8]; cell output [nf]
+  const Cell* cells = nullptr;               // one per cell
+};
 int global_prior_build(Model* m, Cursor& cur);
-int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B);
+int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B,
+                         const GpRecord* rec = nullptr);
 void global_prior_free(GlobalPriorBlk*);
 
 struct Model {

@@ -1938,6 +1938,27 @@ extern "C" int lion_global_prior_forward(LionModel* h, const float* x, const flo
   return two_pass(m, stream, B, [&](Fwd& f) { (void)f; return global_prior_forward(m, x, t, clip, out, B); });
 }
 
+// A global-prior forward as lion_global_prior_forward runs it, with every Linear's output copied out.  taps: 5 + 4 ncell
+// device pointers [B][width] fp32, any of them NULL: pe [emb], t0 [4 emb], temb [nf], cmap [nf] (CLIP models only), h0
+// [nf], then per cell a [nf], bb [nf], s [nf/8], h [nf].
+extern "C" int lion_global_prior_probe(LionModel* h, const float* x, const float* t, const float* clip, float* out,
+                                       void* const* taps, int ntaps, int B, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_GLOBAL_PRIOR, "lion_global_prior_probe: not a global-prior model");
+  LION_REQUIRE(x && t && out && taps && B > 0, "lion_global_prior_probe: bad arguments");
+  Model* m = &h->m;
+  const int ncell = m->desc[3], has_clip = m->desc[4];    // desc: [D, nf, emb, ncell, clip, clip_dim, scale_bits]
+  LION_REQUIRE(ntaps == 5 + 4 * ncell, "lion_global_prior_probe: %d taps given, %d expected", ntaps, 5 + 4 * ncell);
+  LION_REQUIRE(has_clip || !taps[3], "lion_global_prior_probe: a cmap tap for a network without CLIP");
+  GpRecord rec;
+  std::vector<GpRecord::Cell> cells(ncell);
+  int k = 0;
+  auto tap = [&]() { return (float*)taps[k++]; };
+  rec.pe = tap(); rec.t0 = tap(); rec.temb = tap(); rec.cmap = tap(); rec.h0 = tap();
+  for (GpRecord::Cell& cl : cells) { cl.a = tap(); cl.bb = tap(); cl.s = tap(); cl.h = tap(); }
+  rec.cells = cells.data();
+  return two_pass(m, stream, B, [&](Fwd& f) { (void)f; return global_prior_forward(m, x, t, clip, out, B, &rec); });
+}
+
 // ---- measurement hook: time the convolution kernel alone (bench.py roofline leg) ------------
 __global__ void k_fill_pattern(float* p, size_t n, float scale) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

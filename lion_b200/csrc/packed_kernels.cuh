@@ -540,11 +540,12 @@ __global__ void k_small_linear(const float* __restrict__ W, const float* __restr
 // host in float64 and rounded to fp32 exactly like the reference
 __global__ void k_time_sinusoid(const float* __restrict__ t, const float* __restrict__ freqs, float* __restrict__ out,
                                 int half, float scale) {
-  int b = blockIdx.x, i = threadIdx.x;
-  if (i >= half) return;
-  float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);
-  out[(size_t)b * 2 * half + i] = sinf(e);
-  out[(size_t)b * 2 * half + half + i] = cosf(e);
+  const int b = blockIdx.x;
+  for (int i = threadIdx.x; i < half; i += blockDim.x) {     // any time_dim, whatever the block size
+    float e = __fmul_rn(__fmul_rn(t[b], scale), freqs[i]);
+    out[(size_t)b * 2 * half + i] = sinf(e);
+    out[(size_t)b * 2 * half + half + i] = cosf(e);
+  }
 }
 
 // ------------------------------------------------------------------------------------

@@ -314,3 +314,88 @@ def sinusoid(t, E):
 def linear_f64(x, w, b, leaky=False):
     y = x.double() @ w.double().T + b.double()
     return torch.where(y > 0, y, 0.1 * y) if leaky else y
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# global prior (csrc/global_prior.cu): positional embedding, split-K Linears on the tensor cores, SE cells
+#
+# Operand model of k_gp_partial: the activation slice is rounded by the kernel, cvt.rna of fl32(x + add); the weights
+# are staged by cp.async unrounded and handed to mma.sync as fp32 bits, so the tensor core reads them truncated.
+# ---------------------------------------------------------------------------------------------------------------------
+def gp_operand_models(tc=True):
+    """(activation model, weight model) of a global-prior Linear; identities for comparisons with the fp32 oracle."""
+    return (tf32_rna, tf32_trunc) if tc else (_ident, _ident)
+
+
+def gp_freqs(half):
+    """The frequency table global_prior_build computes on the host: expf(fl32(i) * fl32(-log(1e4) / (half - 1))), here
+    as float64 exp of the fp32 argument rounded to fp32 (the correctly rounded expf).  At half = 64 this is the
+    reference's torch.exp table bit for bit; torch's CPU exp (its AVX-512 path) differs from it in 3 of 128 entries at
+    half = 128 and in 1 at half = 32, which depends on the host's instruction set and is not modelled."""
+    step = np.float32(np.log(10000.0) / (half - 1))
+    arg = np.arange(half, dtype=np.float32) * -step
+    return torch.from_numpy(np.exp(arg.astype(np.float64)).astype(np.float32))
+
+
+def gp_posemb(t, emb, scale):
+    """k_gp_posemb in float64 of the kernel's fp32 argument fl32(fl32(t * scale) * freq).  t [B] -> float64 [B, emb]."""
+    tf = t.float().cpu() * torch.tensor(scale, dtype=torch.float32)
+    e = (tf[:, None] * gp_freqs(emb // 2)[None, :]).double()
+    return torch.cat([torch.sin(e), torch.cos(e)], 1)
+
+
+def gp_linear_f64(x, w, b, add=None, tc=True):
+    """One k_gp_partial + k_gp_reduce Linear in float64 on modelled operands: W~ x~ + b with x~ = act(fl32(x + add)) and
+    W~ = wmodel(w).  x, add [B, K] (rounded to fp32 first), w [O, K, ...], b [O] or None.  Returns (y, bound) float64
+    [B, O], bound = |W~| |x~| + |b|: the scale of the sum's rounding error, which no cancellation can hide."""
+    act, wm = gp_operand_models(tc)
+    xs = x.float() if add is None else x.float() + add.float()
+    xt = act(xs).double()
+    wt = wm(w.reshape(w.shape[0], -1).float().contiguous()).double().to(xt.device)
+    y, bound = xt @ wt.T, xt.abs() @ wt.abs().T
+    if b is not None:
+        y, bound = y + b.double().to(xt.device), bound + b.abs().double().to(xt.device)
+    return y, bound
+
+
+def gp_conv1_f64(h, temb, cmap, w, b, tc=True):
+    """A cell's conv1 as the kernel reads it: act(fl32(h + temb)), and for CLIP cells [act(fl32(h + temb)) | act(cmap)]
+    (the cmap half meets the zero half of [temb | 0])."""
+    if cmap is None:
+        return gp_linear_f64(h, w, b, add=temb, tc=tc)
+    return gp_linear_f64(torch.cat([h.float(), cmap.float()], 1), w, b,
+                         add=torch.cat([temb.float(), torch.zeros_like(cmap, dtype=torch.float32)], 1), tc=tc)
+
+
+def gp_cell_out(s, w2, bb, h, tc=True):
+    """k_gp_reduce of SE fc2: sigmoid(W~2 s~) * bb + h, the gate in float64.  Returns (y, bound = |gate bb| + |h|)."""
+    z, _ = gp_linear_f64(s, w2, None, tc=tc)
+    gb = torch.sigmoid(z) * bb.double()
+    return gb + h.double(), gb.abs() + h.double().abs()
+
+
+def gp_forward_f64(sd, x, t, clip=None, emb=128, scale=1.0, tc=True):
+    """The global prior (Prior.forward with SE cells) in float64, the operand model applied to its own activations.
+    Returns {stage: float64 [B, width]} with the probe's tap names (cells as lists) and 'out'."""
+    relu = torch.relu
+    S = {"pe": gp_posemb(t, emb, scale).to(x.device)}
+    S["t0"] = gp_linear_f64(S["pe"], sd["temb_layer.0.weight"], sd["temb_layer.0.bias"], tc=tc)[0]
+    S["temb"] = gp_linear_f64(S["t0"], sd["temb_layer.1.weight"], sd["temb_layer.1.bias"], tc=tc)[0]
+    S["cmap"] = None
+    if clip is not None:
+        S["cmap"] = gp_linear_f64(clip, sd["clip_feat_mapping.weight"], sd["clip_feat_mapping.bias"], tc=tc)[0]
+    h = S["h0"] = gp_linear_f64(x, sd["input_layer.weight"], sd["input_layer.bias"], tc=tc)[0]
+    for n in ("a", "bb", "s", "h"):
+        S[n] = []
+    k = 0
+    while "all_modules.%d.conv1.weight" % k in sd:
+        p = "all_modules.%d." % k
+        a = relu(gp_conv1_f64(h, S["temb"], S["cmap"], sd[p + "conv1.weight"], sd[p + "conv1.bias"], tc=tc)[0])
+        bb = relu(gp_linear_f64(a, sd[p + "conv2.weight"], sd[p + "conv2.bias"], tc=tc)[0])
+        s = relu(gp_linear_f64(bb, sd[p + "SE.fc.0.weight"], None, tc=tc)[0])
+        h = gp_cell_out(s, sd[p + "SE.fc.2.weight"], bb.float(), h.float(), tc=tc)[0]
+        for n, v in zip(("a", "bb", "s", "h"), (a, bb, s, h)):
+            S[n].append(v)
+        k += 1
+    S["out"] = gp_linear_f64(h, sd["output_layer.weight"], sd["output_layer.bias"], tc=tc)[0]
+    return S

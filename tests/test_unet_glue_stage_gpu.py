@@ -40,7 +40,8 @@ TOL_STAGE = 8e-3
 TIMES = [0.0, 1.0, 500.0, 999.0, 1000.0]
 
 
-def _net(kind):
+def _net(kind, E=64):
+    """kind: prior, prior_clip or decoder; E: the prior's time-embedding width (cfg.ddpm.time_dim)."""
     from lion_b200.config import default_prior_cfg
     from lion_b200.models.latent_points_ada import PVCNN2Unet
     clip = kind == "prior_clip"
@@ -50,8 +51,8 @@ def _net(kind):
         net = PVCNN2Unet(3, 0, True, extra_feature_channels=1, input_dim=3, cfg=cfg, sa_blocks=ON.DEC_SA_BLOCKS,
                          fp_blocks=ON.FP_BLOCKS)
     else:
-        spec = ON.prior_spec(clip=clip)
-        net = PVCNN2Unet(4, 64, True, extra_feature_channels=1, input_dim=3, cfg=cfg, sa_blocks=ON.PRIOR_SA_BLOCKS,
+        spec = ON.prior_spec(time_dim=E, clip=clip)
+        net = PVCNN2Unet(4, E, True, extra_feature_channels=1, input_dim=3, cfg=cfg, sa_blocks=ON.PRIOR_SA_BLOCKS,
                          fp_blocks=ON.FP_BLOCKS, clip_forge_enable=clip, clip_forge_dim=cfg.clipforge.feat_dim)
     sd = synth_state_dict({k: list(v.shape) for k, v in net.state_dict().items()}, 41)
     net.load_state_dict(sd)
@@ -213,3 +214,23 @@ def test_unet_glue_stages(kind, B):
     cached, _ = _probe(m, spec, x, t, None, None, len(layers), total)
     assert torch.equal(cached["aff"], P["aff"]), "cached style affines differ from the inline ones"
     assert torch.equal(cached["out"], P["out"]), "output with the cached style differs from the inline style"
+
+
+@pytest.mark.parametrize("E", [256])
+def test_unet_time_embedding_wide(E):
+    """A prior U-Net with time_dim = 256: 128 frequencies, more than the 64 threads k_time_sinusoid is launched with.
+    The sinusoid and the two time-embedding Linears against float64, each from the probe's previous stage."""
+    net, sd, spec, cfg = _net("prior", E)
+    m = L.model_for(net, L.KIND_UNET, net.lion_desc(), net.lion_params())
+    B = 2
+    x = gen(90, B, N, 4, scale=0.4).cuda()
+    t = torch.tensor([999.0, 1000.0], device="cuda")
+    style = gen(91, B, cfg.latent_pts.style_dim).cuda()
+    layers = _emd_layers(sd)
+    P, _ = _probe(m, spec, x, t, style, None, len(layers), sum(2 * c for _, c in layers))
+    e = {"sinu": (P["sinu"].double() - SR.sinusoid(t, E).cuda()).abs().max().item()}
+    e["h"] = _rel(P["h"], SR.linear_f64(P["sinu"], sd["embedf.0.weight"], sd["embedf.0.bias"], leaky=True), (0, 1))
+    e["temb"] = _rel(P["temb"], SR.linear_f64(P["h"], sd["embedf.2.weight"], sd["embedf.2.bias"]), (0, 1))
+    print("unet time embedding E=%d: %s" % (E, ", ".join("%s %.2e" % kv for kv in e.items())), flush=True)
+    assert e["sinu"] <= TOL_SINU and max(e["h"], e["temb"]) <= TOL_LINEAR, e
+    assert torch.equal(net.forward_point_major(x, t=t, style=style), P["out"]), "probe output differs from lion_unet_forward"
