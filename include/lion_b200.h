@@ -273,6 +273,60 @@ int lion_ddim_set_step(int* step_ptr, float* t_out, const float* tables, int B, 
 int lion_ddim_next_step(int* step_ptr, float* t_out, const float* tables, int B, int S, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Device-resident adaptive RK45 for the probability-flow ODE of the VPSDE (utils/diffusion_continuous.py:90-176
+ * compute_ode_nll and :178-249 sample_model_ode, both through scipy's RK45 as solve_ivp(..., t_eval=...) drives it:
+ * scipy/integrate/_ivp/rk.py RungeKutta._step_impl, rk_step, the RK45 tableaux and RkDenseOutput; common.py
+ * select_initial_step and norm).  The integration variable s runs from t0 to t_bound (either direction); the model
+ * sees t = s, or t = -s with the right-hand side negated when `negate` is set (torchdiffeq's treatment of a
+ * decreasing time span).  All integrator state is on the device:
+ *   st  one LionOdeState (below), written by these calls only;
+ *   y, y_new [n] float64; K [7][n] float64 (the stages, K[6] = f at the step's end); partials [2][256] float64;
+ *   x [n] fp32 the model input of the current evaluation, t_model [B] fp32 its time (every row the same).
+ * One evaluation = lion_ode_stage (x, t_model) -> the caller's model forward (eps [n] fp32) -> lion_ode_rhs.
+ * Driver: lion_ode_init; evaluation of stage 0; lion_ode_norms/control(LION_ODE_INIT_H0); evaluation of stage
+ * LION_ODE_STAGE_PROBE; lion_ode_norms/control(LION_ODE_INIT_H1); then per step attempt: lion_ode_control(BEGIN),
+ * evaluations of stages 1..6, lion_ode_norms/control(END), lion_ode_commit -- until st->status != RUNNING; then
+ * lion_ode_dense_end.  Every call after lion_ode_init reads the status on the device and does nothing once the
+ * integration stopped, so a captured step attempt can be replayed without host-side parameters.
+ * Sums run in a fixed order without FMA contraction and the norms reduce fixed-size partials in a fixed order:
+ * results are bit-reproducible.  Requires n > 0 and B > 0.
+ * ------------------------------------------------------------------------------------- */
+enum { LION_ODE_RUNNING = 0, LION_ODE_DONE = 1, LION_ODE_TOO_SMALL = 2 };
+enum { LION_ODE_INIT_H0 = 0, LION_ODE_INIT_H1 = 1, LION_ODE_END = 2, LION_ODE_BEGIN = 3 };
+#define LION_ODE_STAGE_PROBE 7     /* the second evaluation of select_initial_step: y0 + h0 * direction * f0 */
+typedef struct LionOdeState {
+  double t, t_bound, direction, rtol, atol;
+  double h_abs;                    /* scipy's self.h_abs, the loop-local h_abs during a step attempt */
+  double h, t_new, min_step;       /* the current attempt */
+  double h0, d1, err_norm;         /* select_initial_step; the last attempt's error norm */
+  int status, nfe, n_accepted, n_rejected;
+  int step_rejected, new_step, accepted, negate;
+} LionOdeState;
+size_t lion_ode_state_bytes(void);
+/* st <- start at t0 (y = y0 widened, rtol / atol as given, nfe = 0; status DONE when t0 == t_bound) */
+int lion_ode_init(LionOdeState* st, const float* y0, double* y, size_t n, double t0, double t_bound, double rtol,
+                  double atol, int negate, void* stream);
+/* x <- the model input of `stage` rounded to fp32, t_model[0..B) <- float32(+-(t + c_stage h)); stage 6 also writes
+ * y_new.  stage 0: y at t; 1..5: y + (sum_j a_sj K_j) h; 6: y + h sum_j b_j K_j at t + h; LION_ODE_STAGE_PROBE. */
+int lion_ode_stage(LionOdeState* st, const double* y, double* y_new, const double* K, size_t n, int stage, float* x,
+                   float* t_model, int B, void* stream);
+/* K[stage] <- (+-) (f(t) x + ((0.5 g2(t)) eps) / sqrt(var(t))) in fp32, widened; t = t_model[0]; the probe writes
+ * K[1].  beta_start, beta_end, sigma2_0: the VPSDE's (utils/diffusion_continuous.py:571-621); nfe += 1. */
+int lion_ode_rhs(LionOdeState* st, const float* x, const float* eps, double* K, size_t n, int stage, double beta_start,
+                 double beta_end, double sigma2_0, const float* t_model, void* stream);
+/* fixed-order partial sums of squares for the norm that lion_ode_control(`what`) consumes */
+int lion_ode_norms(const LionOdeState* st, const double* y, const double* y_new, const double* K, size_t n, int what,
+                   double* partials, void* stream);
+/* the step-size controller, one thread: what = INIT_H0 / INIT_H1 (select_initial_step), BEGIN (min_step, clamp to
+ * t_bound, too-small check), END (accept / reject, SAFETY 0.9, factors 0.2 .. 10, exponent -1/5) */
+int lion_ode_control(LionOdeState* st, const double* partials, size_t n, int what, void* stream);
+/* after END: on an accepted step that did not finish, y <- y_new and K[0] <- K[6] (FSAL) */
+int lion_ode_commit(const LionOdeState* st, double* y, const double* y_new, double* K, size_t n, void* stream);
+/* out [n] fp32 <- the last step's dense-output polynomial at its end point (RkDenseOutput at x = 1), which is what
+ * solve_ivp returns for t_eval = t_bound; y holds the step's start (lion_ode_commit leaves it on the last step) */
+int lion_ode_dense_end(const LionOdeState* st, const double* y, const double* K, size_t n, float* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * One step of the diffusers-style DDPM scheduler used by LION.sample (models/lion.py:24-26,:55,:70;
  * the scheduler itself is the un-vendored dependency diffusers==0.11.1 -- its published
  * DDPMScheduler.step is restated, PARITY UNPINNED, see DESIGN.md section 2):

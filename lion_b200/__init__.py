@@ -14,7 +14,9 @@ host-side mirror of the reference's Python interface for that path:
     lion_b200.trainers.train_2prior             generate_samples_vada_2prior (DDPM, DDIM and ODE routes)
     lion_b200.trainers.train_prior              Trainer.sample / Trainer.eval_sample (sampling-side Trainer)
     lion_b200.models.pvcnn2 / .shapelatent_modules / .distributions          VAE encoder path (non-Ada blocks)
-    lion_b200.utils.diffusion_continuous        VPSDE + probability-flow ODE sampler
+    lion_b200.utils.diffusion_continuous        VPSDE, probability-flow ODE sampler and encoder (compute_ode_nll)
+    lion_b200.trainers.interpolate_latent       latent interpolation by ODE sampling (script/interpolate.sh)
+    lion_b200.trainers.encode_interp_interp     interpolation between encoded shapes (script/interpolate_posterior.sh)
 
 `lion_b200.install()` registers these under the reference's own import paths (`models.*`,
 `utils.diffusion_pvd`, `trainers.train_2prior`, `third_party.pvcnn.functional`) so that
@@ -45,6 +47,8 @@ _ALIASES = {
     "utils.diffusion_pvd": "lion_b200.utils.diffusion_pvd",
     "utils.diffusion_continuous": "lion_b200.utils.diffusion_continuous",
     "trainers.train_2prior": "lion_b200.trainers.train_2prior",
+    "trainers.interpolate_latent": "lion_b200.trainers.interpolate_latent",
+    "trainers.encode_interp_interp": "lion_b200.trainers.encode_interp_interp",
 }
 
 

@@ -23,7 +23,7 @@ c_f = C.c_void_p   # device pointers travel as integers
 
 
 def _proto(lib):
-    i, f, sz, vp = C.c_int, C.c_float, C.c_size_t, C.c_void_p
+    i, f, d, sz, vp = C.c_int, C.c_float, C.c_double, C.c_size_t, C.c_void_p
     P = lambda *a: list(a)
     sig = {
         "lion_version": ([], i),
@@ -86,6 +86,14 @@ def _proto(lib):
         "lion_ddim_set_step": (P(vp, vp, vp, i, i, i, vp), i),
         "lion_ddim_next_step": (P(vp, vp, vp, i, i, vp), i),
         "lion_scheduler_step": (P(vp, vp, vp, vp, vp, vp, sz, vp), i),
+        "lion_ode_state_bytes": ([], sz),
+        "lion_ode_init": (P(vp, vp, vp, sz, d, d, d, d, i, vp), i),
+        "lion_ode_stage": (P(vp, vp, vp, vp, sz, i, vp, vp, i, vp), i),
+        "lion_ode_rhs": (P(vp, vp, vp, vp, sz, i, d, d, d, vp, vp), i),
+        "lion_ode_norms": (P(vp, vp, vp, vp, sz, i, vp, vp), i),
+        "lion_ode_control": (P(vp, vp, sz, i, vp), i),
+        "lion_ode_commit": (P(vp, vp, vp, vp, sz, vp), i),
+        "lion_ode_dense_end": (P(vp, vp, vp, sz, vp, vp), i),
         "lion_chamfer_forward": (P(vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
         "lion_chamfer_pairwise": (P(vp, vp, vp, i, i, i, i, vp), i),
         "lion_chamfer_backward": (P(vp, vp, vp, vp, vp, vp, vp, vp, i, i, i, vp), i),
@@ -144,6 +152,19 @@ def stream():
 
 
 FWD_CONV_FP16 = 1     # LION_FWD_CONV_FP16 (include/lion_b200.h)
+
+# the device-resident RK45 (include/lion_b200.h: LionOdeState and the lion_ode_* entry points)
+ODE_RUNNING, ODE_DONE, ODE_TOO_SMALL = 0, 1, 2
+ODE_INIT_H0, ODE_INIT_H1, ODE_END, ODE_BEGIN = 0, 1, 2, 3
+ODE_STAGE_PROBE = 7
+ODE_PARTIALS = 2 * 256
+
+
+class OdeState(C.Structure):
+    _fields_ = [(k, C.c_double) for k in ("t", "t_bound", "direction", "rtol", "atol", "h_abs", "h", "t_new", "min_step",
+                                          "h0", "d1", "err_norm")] + \
+               [(k, C.c_int) for k in ("status", "nfe", "n_accepted", "n_rejected", "step_rejected", "new_step", "accepted",
+                                       "negate")]
 
 
 def forward_flags():

@@ -88,6 +88,7 @@ struct UnetBlk {
   const float *e0w = nullptr, *e0b = nullptr, *e2w = nullptr, *e2b = nullptr;
   const float *cfw = nullptr, *cfb = nullptr, *scw = nullptr, *scb = nullptr;
   float* d_freqs = nullptr;
+  float time_scale = 1.0f;                                // sde.embedding_scale: t is scaled before the sinusoid
   std::vector<std::vector<Block>> sa, fp;
   std::vector<UnetLevel> levels;                          // [n_sa]
   cudaEvent_t aux_start = nullptr, temb_done = nullptr;   // the side stream may start; the time embedding is done

@@ -972,6 +972,9 @@ static int build_unet(Model* m, Cursor& cur) {
     }
     u.fp.push_back(std::move(blocks));
   }
+  int scale_bits;
+  if (!rd(scale_bits)) { set_error("unet descriptor truncated (time-embedding scale)"); return LION_ERR_ARG; }
+  memcpy(&u.time_scale, &scale_bits, sizeof(float));
   // per point level: the voxel preps of the PVConvs on its points (SA level l's, then FP stage n_sa - 1 - l's) and the
   // events of what the side stream computes for it
   u.levels.resize(n_sa);
@@ -1090,7 +1093,7 @@ static int unet_side_stream(Fwd& f, const float* t, float* temb, std::vector<Lev
       float* sinu = c->alloc_n<float>((size_t)B * E);
       float* h = c->alloc_n<float>((size_t)B * E);
       if (f.ur) { f.ur->a_sinu = sinu; f.ur->a_h = h; }
-      LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, sinu, E / 2, 1.0f);
+      LION_LAUNCH_ON(c, c->aux, k_time_sinusoid, B, 64, 0, t, u.d_freqs, sinu, E / 2, u.time_scale);
       LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e0w, u.e0b, sinu, E, h, E, E, E, 1);
       LION_LAUNCH_ON(c, c->aux, k_small_linear, B, 128, E * sizeof(float), u.e2w, u.e2b, h, E, temb, E, E, E, 0);
       stamp(c, c->aux, "temb");

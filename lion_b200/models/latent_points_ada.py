@@ -25,7 +25,6 @@ class PVCNN2Unet(nn.Module):
                  clip_forge_enable=0, clip_forge_dim=512):
         super().__init__()
         assert width_multiplier == 1 and voxel_resolution_multiplier == 1
-        assert time_emb_scales == 1.0, "lion_b200: sde.embedding_scale must be 1.0 (all shipped prior configs)"
         self.input_dim = input_dim
         self.clip_forge_enable = clip_forge_enable
         self.clip_forge_dim = clip_forge_dim
@@ -75,6 +74,7 @@ class PVCNN2Unet(nn.Module):
         for fp_cfg, conv_cfg in self.fp_blocks:
             oc, nblk, res = conv_cfg if conv_cfg is not None else (0, 0, 0)
             d += [len(fp_cfg)] + list(fp_cfg) + [int(conv_cfg is not None), oc, nblk, res]
+        d.append(L.float_bits(self.time_emb_scales))       # sde.embedding_scale: t * scale enters the sinusoid
         return d
 
     def lion_params(self):
