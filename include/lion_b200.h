@@ -233,6 +233,30 @@ int lion_global_prior_probe(LionModel* m, const float* x, const float* t, const 
 /* the same call under the name SURVEY.md 8(b) lists (one denoising-step evaluation of the global prior) */
 int lion_global_prior_step(LionModel* m, const float* x, const float* t, const float* clip, float* out, int B,
                            void* stream);
+/* Training the global prior.  lion_global_prior_saved_floats: the size in floats of the buffer the training forward
+ * fills for the backward (0 for a bad model or B).  Its layout, [B][width] fp32 tensors back to back: x [D], pe [emb],
+ * t0 [4*emb], temb [nf], cmap [nf] (CLIP networks only), h0 [nf], then per cell a [nf] (conv1 + ReLU, times the dropout
+ * mask), bb [nf], s [nf/8], gate [nf] (sigmoid(fc2)), h [nf] (the cell output). */
+size_t lion_global_prior_saved_floats(LionModel* m, int B);
+/* lion_global_prior_forward with the dropout of ResBlockSEDrop applied and the saved buffer filled.  drop_mask
+ * [ncell][B][nf] fp32: the scaled mask (0 or 1/(1-p)) multiplied into each cell's conv1 + ReLU output, or NULL for no
+ * dropout, in which case out has the bits lion_global_prior_forward gives. */
+int lion_global_prior_forward_train(LionModel* m, const float* x, const float* t, const float* clip,
+                                    const float* drop_mask, float* saved, float* out, int B, void* stream);
+/* The backward of the training forward that filled `saved` (same model, clip, drop_mask and B; the parameters unchanged
+ * since): from gout [B][D] = dL/d out, writes gx [B][D] = dL/d x and gparams[i] = dL/d params[i] for every parameter
+ * in the order lion_model_create took them (nparams of them; each is overwritten, not accumulated).  No gradient
+ * reaches t or clip.  Deterministic: no atomics, every sum in a fixed order. */
+int lion_global_prior_backward(LionModel* m, const float* saved, const float* clip, const float* drop_mask,
+                               const float* gout, float* gx, float* const* gparams, int nparams, int B, void* stream);
+/* lion_global_prior_backward with the gradients between the Linears copied into caller buffers.  taps holds
+ * 4 + 5*ncell device pointers [B, width] fp32, each may be NULL: gtemb [nf] (dL/d temb, summed over the cells),
+ * gt0 [4*emb] (dL/d t0), gcmap [nf] (dL/d clip_feat_mapping output; CLIP networks only), gh0 [nf] (dL/d h0);
+ * per cell: gh [nf] (dL/d cell output), gz [nf] (dL/d fc2 before the sigmoid), gs [nf/8] (dL/d fc0 before its ReLU),
+ * gbb [nf] (dL/d conv2 before its ReLU), gz1 [nf] (dL/d conv1 before its ReLU).  taps = NULL: no copies. */
+int lion_global_prior_backward_probe(LionModel* m, const float* saved, const float* clip, const float* drop_mask,
+                                     const float* gout, float* gx, float* const* gparams, int nparams,
+                                     void* const* taps, int ntaps, int B, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * One ancestral DDPM step (utils/diffusion_pvd.py:283-296 + :475-486), elementwise over n.

@@ -81,6 +81,10 @@ def _proto(lib):
         "lion_unet_probe": (P(vp, vp, vp, vp, vp, vp, C.POINTER(vp), i, C.POINTER(i), i, i, i, vp), i),
         "lion_global_prior_step": (P(vp, vp, vp, vp, vp, i, vp), i),
         "lion_global_prior_probe": (P(vp, vp, vp, vp, vp, C.POINTER(vp), i, i, vp), i),
+        "lion_global_prior_saved_floats": (P(vp, i), sz),
+        "lion_global_prior_forward_train": (P(vp, vp, vp, vp, vp, vp, vp, i, vp), i),
+        "lion_global_prior_backward": (P(vp, vp, vp, vp, vp, vp, C.POINTER(vp), i, i, vp), i),
+        "lion_global_prior_backward_probe": (P(vp, vp, vp, vp, vp, vp, C.POINTER(vp), i, C.POINTER(vp), i, i, vp), i),
         "lion_workspace_bytes": (P(vp), sz),
         "lion_ddim_update": (P(vp, vp, vp, vp, vp, vp, sz, vp, vp), i),
         "lion_ddim_set_step": (P(vp, vp, vp, i, i, i, vp), i),

@@ -107,12 +107,28 @@ struct GlobalPriorBlk;   // global_prior.cu
 // the stream right after the Linear that produced it (real pass only; never set in a product call).  Any may be null.
 struct GpRecord {
   float *pe = nullptr, *t0 = nullptr, *temb = nullptr, *cmap = nullptr, *h0 = nullptr;   // [emb], [4 emb], [nf] x 3
-  struct Cell { float *a, *bb, *s, *h; };   // conv1 + ReLU, conv2 + ReLU [nf]; SE fc0 + ReLU [nf/8]; cell output [nf]
+  // conv1 + ReLU (+ dropout), conv2 + ReLU [nf]; SE fc0 + ReLU [nf/8]; cell output [nf]; SE gate sigmoid(fc2) [nf]
+  // (gate: written by the reduce itself, not copied, and only by the training forward)
+  struct Cell { float *a, *bb, *s, *h, *gate; };
   const Cell* cells = nullptr;               // one per cell
+};
+// Caller buffers ([B][width] fp32) that lion_global_prior_backward_probe has global_prior_backward fill with the
+// gradients flowing between the Linears.  Any may be null.
+struct GpBwdRecord {
+  float *gtemb = nullptr, *gt0 = nullptr, *gcmap = nullptr, *gh0 = nullptr;   // [nf], [4 emb], [nf], [nf]
+  // d/d(cell output) [nf]; d/d(fc2 pre-sigmoid) [nf]; d/d(fc0 pre-ReLU) [nf/8]; d/d(conv2 pre-ReLU) [nf];
+  // d/d(conv1 pre-ReLU) [nf]
+  struct Cell { float *gh, *gz, *gs, *gbb, *gz1; };
+  const Cell* cells = nullptr;
 };
 int global_prior_build(Model* m, Cursor& cur);
 int global_prior_forward(Model* m, const float* x, const float* t, const float* clip, float* out, int B,
-                         const GpRecord* rec = nullptr);
+                         const GpRecord* rec = nullptr, const float* drop = nullptr);
+size_t global_prior_saved_floats(const Model* m, int B);
+int global_prior_forward_train(Model* m, const float* x, const float* t, const float* clip, const float* drop,
+                               float* saved, float* out, int B);
+int global_prior_backward(Model* m, const float* saved, const float* clip, const float* drop, const float* gout,
+                          float* gx, const float* const* gparams, int nparams, int B, const GpBwdRecord* rec = nullptr);
 void global_prior_free(GlobalPriorBlk*);
 
 struct Model {

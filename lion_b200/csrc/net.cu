@@ -1962,6 +1962,54 @@ extern "C" int lion_global_prior_probe(LionModel* h, const float* x, const float
   return two_pass(m, stream, B, [&](Fwd& f) { (void)f; return global_prior_forward(m, x, t, clip, out, B, &rec); });
 }
 
+extern "C" size_t lion_global_prior_saved_floats(LionModel* h, int B) {
+  if (!h || h->m.kind != LION_KIND_GLOBAL_PRIOR || B <= 0) return 0;
+  return global_prior_saved_floats(&h->m, B);
+}
+
+extern "C" int lion_global_prior_forward_train(LionModel* h, const float* x, const float* t, const float* clip,
+                                               const float* drop_mask, float* saved, float* out, int B, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_GLOBAL_PRIOR, "lion_global_prior_forward_train: not a global-prior model");
+  LION_REQUIRE(x && t && saved && out && B > 0, "lion_global_prior_forward_train: bad arguments");
+  Model* m = &h->m;
+  return two_pass(m, stream, B, [&](Fwd& f) { (void)f; return global_prior_forward_train(m, x, t, clip, drop_mask, saved, out, B); });
+}
+
+extern "C" int lion_global_prior_backward(LionModel* h, const float* saved, const float* clip, const float* drop_mask,
+                                          const float* gout, float* gx, float* const* gparams, int nparams, int B,
+                                          void* stream) {
+  return lion_global_prior_backward_probe(h, saved, clip, drop_mask, gout, gx, gparams, nparams, nullptr, 0, B, stream);
+}
+
+// The backward as lion_global_prior_backward runs it, with the gradients between the Linears copied out.  taps: 4 + 5 ncell
+// device pointers [B][width] fp32, any of them NULL: gtemb [nf], gt0 [4 emb], gcmap [nf] (CLIP models only), gh0 [nf],
+// then per cell gh [nf], gz [nf], gs [nf/8], gbb [nf], gz1 [nf].
+extern "C" int lion_global_prior_backward_probe(LionModel* h, const float* saved, const float* clip, const float* drop_mask,
+                                                const float* gout, float* gx, float* const* gparams, int nparams,
+                                                void* const* taps, int ntaps, int B, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_GLOBAL_PRIOR, "lion_global_prior_backward: not a global-prior model");
+  LION_REQUIRE(saved && gout && gx && gparams && B > 0, "lion_global_prior_backward: bad arguments");
+  for (int i = 0; i < nparams; ++i) LION_REQUIRE(gparams[i], "lion_global_prior_backward: gradient %d is null", i);
+  Model* m = &h->m;
+  const int ncell = m->desc[3], has_clip = m->desc[4];
+  GpBwdRecord rec;
+  std::vector<GpBwdRecord::Cell> cells(ncell);
+  if (taps) {
+    LION_REQUIRE(ntaps == 4 + 5 * ncell, "lion_global_prior_backward_probe: %d taps given, %d expected", ntaps, 4 + 5 * ncell);
+    LION_REQUIRE(has_clip || !taps[2], "lion_global_prior_backward_probe: a gcmap tap for a network without CLIP");
+    int k = 0;
+    auto tap = [&]() { return (float*)taps[k++]; };
+    rec.gtemb = tap(); rec.gt0 = tap(); rec.gcmap = tap(); rec.gh0 = tap();
+    for (GpBwdRecord::Cell& cl : cells) { cl.gh = tap(); cl.gz = tap(); cl.gs = tap(); cl.gbb = tap(); cl.gz1 = tap(); }
+    rec.cells = cells.data();
+  }
+  return two_pass(m, stream, B, [&](Fwd& f) {
+    (void)f;
+    return global_prior_backward(m, saved, clip, drop_mask, gout, gx, (const float* const*)gparams, nparams, B,
+                                 taps ? &rec : nullptr);
+  });
+}
+
 // ---- measurement hook: time the convolution kernel alone (bench.py roofline leg) ------------
 __global__ void k_fill_pattern(float* p, size_t n, float scale) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

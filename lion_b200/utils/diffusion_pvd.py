@@ -69,6 +69,39 @@ class DiffusionDiscretized(object):
         return None
 
     # ------------------------------------------------------------------------------------
+    # training objective (diffusion_pvd.py:44-113): the quantities train_2prior.train_iter draws for its prior losses
+    def _iw_at(self, B, timestep):
+        """timestep int64 [B] in [1, T] -> (timestep, var_t [B,1,1,1] = 1 - alpha_bar, m_t [B,1,1,1] = sqrt(alpha_bar),
+        loss weight (the p2 weight 1 / (p2_k + snr)^p2_gamma [B] with ddpm.use_p2_weight, 1.0 otherwise), None, None)"""
+        alpha_bars = torch.gather(self._alpha_bars, 0, timestep - 1)
+        var_t = (1.0 - alpha_bars)[:, None, None, None]
+        m_t = torch.sqrt(alpha_bars)[:, None, None, None]
+        loss_weight = 1.0
+        if self.use_p2_weight:
+            loss_weight = torch.gather(1 / (self.p2_k + self.snr) ** self.p2_gamma, 0, timestep - 1).view(B)
+        return timestep, var_t, m_t, loss_weight, None, None
+
+    def iw_quantities(self, B, *args):
+        """Diffusion quantities at B timesteps drawn uniformly from {1, .., T}: floor(U[0, 1) * T) + 1 with U from
+        torch.rand on this object's device (the reference draws on 'cuda').  Extra arguments (time_eps, iw_sample_p,
+        iw_subvp_like_vp_sde in the reference's call) are ignored, as there."""
+        rho = torch.rand(size=[B], device=self._alpha_bars.device) * self._diffusion_steps
+        timestep = rho.type(torch.int64)
+        assert timestep.max() <= self._diffusion_steps - 1, 'get max at %d' % timestep.max()
+        return self._iw_at(B, timestep + 1)
+
+    def iw_quantities_t(self, B, timestep, *args):
+        """iw_quantities at given 0-based timesteps [B] (int64, in [0, T-1])."""
+        return self._iw_at(B, timestep.view(B) + 1)
+
+    def sample_q(self, x_init, noise, var_t, m_t):
+        """A draw of the forward process at t: m_t * x_init + sqrt(var_t) * noise, all 4-D ([B, C, 1, 1], var_t and m_t
+        [B, 1, 1, 1] as iw_quantities returns them)."""
+        assert len(x_init.shape) == 4 and len(var_t.shape) == 4 and len(m_t.shape) == 4
+        assert x_init.shape[0] == m_t.shape[0]
+        return m_t * x_init + torch.sqrt(var_t) * noise
+
+    # ------------------------------------------------------------------------------------
     def _step_tables(self, device):
         """[T][4] fp32 rows consumed by lion_ddpm_update, built with the reference's own fp32
         expressions (diffusion_pvd.py:161, :475-486)."""
