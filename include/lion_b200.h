@@ -33,6 +33,11 @@ int lion_ctx_last_conv_stage_taps(LionCtx* ctx);
 /* For tests: on != 0 makes every later 3x3x3 convolution on this context stream whole weight slabs (the outputs are
  * bitwise the same either way; only the shared-memory rings differ); 0 restores the automatic choice.  Returns 0. */
 int lion_ctx_set_conv_whole_slabs(LionCtx* ctx, int on);
+/* For tests: on != 0 makes the sparse first convolution of every later PVConv on this context store its whole raw
+ * output and the activation pass after it read every interior position, as before the activity mask existed (the
+ * outputs are bitwise the same either way); 0 restores the default, which stores and reads only voxels with an occupied
+ * neighbour.  Returns 0. */
+int lion_ctx_set_sparse_conv1_dense(LionCtx* ctx, int on);
 /* Scratch-arena generation: bumped whenever a call had to re-allocate the per-device arena or zero grid.  A CUDA graph
  * captured on this context has the arena addresses baked in; it must not be replayed once the generation changed
  * (lion_b200._lib.capture_graph checks this and raises). */
@@ -174,6 +179,12 @@ int lion_conv3d_gn_fwd_flags(LionModel* m, const float* x, float* out, double* g
  * (may be NULL) = 1 (dense) or 2 (sparse). */
 int lion_pvconv_conv1_probe(LionModel* m, const float* features, const float* coords, int path, float* out,
                             double* gn_sum, double* gn_sqsum, int* path_taken, int B, int N, void* stream);
+/* lion_pvconv_conv1_mask_probe: the sparse first convolution's voxel ids and activity mask.  vgrid [B,r+2,r+2,r+2]
+ * int32 = compact id of the occupied voxel at each (haloed) position, -1 where empty; mask [B,ceil(r^3/32)] uint32, bit j
+ * of word w set when interior voxel 32 w + j (x-major, z fastest) has an occupied voxel among its 27 neighbours.  An
+ * error where the sparse path cannot serve the layer. */
+int lion_pvconv_conv1_mask_probe(LionModel* m, const float* features, const float* coords, int* vgrid, unsigned* mask, int B,
+                                 int N, void* stream);
 /* lion_sa_mlp_probe: an SA model's MLP.  path: 0 = the path lion_sa_module_fwd chooses, 1 = unfused kernels, 2 = fused.
  * Per layer l with C_l channels, at offset B * (C_0 + ... + C_{l-1}): gn_sum / gn_sqsum [B,C_l] (doubles) and the folded
  * AdaGN scale / shift [B,C_l]; pool_mm [B][C_last/4][M][2][4] the minimum (index 0) and maximum (1) of the last layer's

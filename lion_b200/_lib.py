@@ -34,6 +34,7 @@ def _proto(lib):
         "lion_ctx_last_conv_group": (P(vp), i),
         "lion_ctx_last_conv_stage_taps": (P(vp), i),
         "lion_ctx_set_conv_whole_slabs": (P(vp, i), i),
+        "lion_ctx_set_sparse_conv1_dense": (P(vp, i), i),
         "lion_ctx_arena_bytes": (P(vp), sz),
         "lion_ctx_generation": (P(vp), C.c_uint),
         "lion_ctx_timeline": (P(vp, vp, vp, i), i),
@@ -73,6 +74,7 @@ def _proto(lib):
         "lion_conv3d_gn_fwd": (P(vp, vp, vp, vp, vp, i, vp), i),
         "lion_conv3d_gn_fwd_flags": (P(vp, vp, vp, vp, vp, i, i, vp), i),
         "lion_pvconv_conv1_probe": (P(vp, vp, vp, i, vp, vp, vp, C.POINTER(i), i, i, vp), i),
+        "lion_pvconv_conv1_mask_probe": (P(vp, vp, vp, vp, vp, i, i, vp), i),
         "lion_sa_mlp_probe": (P(vp, vp, vp, vp, i, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
         "lion_pvconv_probe": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, vp), i),
         "lion_pvconv_probe_flags": (P(vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i), i, i, i, vp), i),

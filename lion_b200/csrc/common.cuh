@@ -75,6 +75,9 @@ struct Ctx {
   int conv_stage_taps = 0;
   // set by tests only (lion_ctx_set_conv_whole_slabs): 3x3x3 weight slabs are always streamed whole
   bool conv_whole_slabs = false;
+  // set by tests only (lion_ctx_set_sparse_conv1_dense): the sparse first convolution stores every voxel of its output
+  // and the activation pass reads every interior position (no activity mask)
+  bool sparse_conv1_dense = false;
   // LION_TIMELINE=1 (diagnostic, tools/timeline_step.py): %globaltimer stamps dropped into both streams at block
   // boundaries -- this image has no nsys, and a step's critical path across the two streams is not visible otherwise
   unsigned long long* d_stamps = nullptr;

@@ -584,10 +584,14 @@ static int get_vox(Fwd& f, cudaStream_t s, const float4* c4, int N, int r, VoxPr
 // path: 0 = the product's choice (sparse when the grid is sparse enough and the wide packing serves it), 1 = the dense
 // tensor-core convolution with occupancy skip, 2 = sparse.  A dense run leaves the scattered voxels in the context's zero
 // grid (g_in): the caller restores it (k_act_grid's extra blocks).  after_scatter() runs between the scatter and the
-// convolution (pvconv_fwd launches its point branch there).
-struct Conv1Out { float4* raw = nullptr; double* ssum = nullptr; double* ssq = nullptr; float4* g_in = nullptr; bool sparse = false; };
+// convolution (pvconv_fwd launches its point branch there).  A sparse run stores only the voxels its activity mask marks
+// (the rest hold exactly the bias, which k_act_grid substitutes) unless whole_raw: then the raw output is stored whole.
+// o.mask: the activity mask of a sparse run, [B][ceil(r^3 / 32)] words (null after a dense run).
+struct Conv1Out { float4* raw = nullptr; double* ssum = nullptr; double* ssq = nullptr; float4* g_in = nullptr; bool sparse = false;
+                  const unsigned* mask = nullptr; };
 template <typename F>
-static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, int path, Conv1Out& o, F&& after_scatter) {
+static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, int path, bool whole_raw, Conv1Out& o,
+                        F&& after_scatter) {
   const int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
   ConvGeom geo1 = geom_grid(r);
   // (the tensor-core kernel still skips operand slabs whose 64-row occupancy flags are all clear)
@@ -635,12 +639,17 @@ static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, 
       LION_CHECK_CUDA(cudaFuncSetAttribute(k_scatter_compact, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
     const dim3 grid(cdiv(r * r * r, 32 * nwarp), f.B);
+    unsigned* mask = f.c->alloc_n<unsigned>((size_t)f.B * cdiv(r * r * r, 32));
+    const bool whole = whole_raw || f.c->sparse_conv1_dense;
     if (p.c1.cout_pad == 32)
-      LION_LAUNCH(f.c, k_sparse_conv_gather<32>, grid, 32 * nwarp, smem, y, ld, vp->vgrid, p.c1.bias, raw1, s1, q1, p.c1.cout_pad, r, N);
+      LION_LAUNCH(f.c, k_sparse_conv_gather<32>, grid, 32 * nwarp, smem, y, ld, vp->vgrid, p.c1.bias, raw1, s1, q1, p.c1.cout_pad, r, N,
+                  mask, whole);
     else
-      LION_LAUNCH(f.c, k_sparse_conv_gather<64>, grid, 32 * nwarp, smem, y, ld, vp->vgrid, p.c1.bias, raw1, s1, q1, p.c1.cout_pad, r, N);
+      LION_LAUNCH(f.c, k_sparse_conv_gather<64>, grid, 32 * nwarp, smem, y, ld, vp->vgrid, p.c1.bias, raw1, s1, q1, p.c1.cout_pad, r, N,
+                  mask, whole);
     LION_TRY(check_launch(f.c, "sparse conv1"));
     o.ssum = s1; o.ssq = q1;
+    o.mask = mask;
   } else {
     LION_TRY(alloc_stats(f, p.c1.cout_pad, &o.ssum, &o.ssq));
     LION_TRY(run_conv(f, p.c1, o.g_in, Gin, raw1, Gout, o.ssum, o.ssq, geo1));
@@ -663,12 +672,13 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   // scatter -> point branch -> conv1 -> (stats) -> AdaGN + Swish.  The point branch is conv1x1 -> stats (its fold shares
   // a launch with conv1's below; the activation is applied inside the devox kernel).
   Conv1Out c1;
-  LION_TRY(pvconv_conv1(f, p, feat, vp, 0, c1, [&]() -> int {
+  LION_TRY(pvconv_conv1(f, p, feat, vp, 0, f.pv != nullptr, c1, [&]() -> int {
     rawp = alloc_pf(f, Gout, N);
     return conv_gn_deferred(f, pw, feat.p, feat.G, rawp.p, Gout, geom_rows(N), p.point.gn[0], (double)N, ap, jp);
   }));
   const bool sparse1 = c1.sparse;
   float4 *raw1 = c1.raw, *g_in = c1.g_in;
+  const unsigned* mask1 = f.c->sparse_conv1_dense ? nullptr : c1.mask;     // (null: k_act_grid reads every position)
   AffSrc a1;
   const double V = (double)r * r * r;
   j1 = prep_job(f, p.g1, c1.ssum, c1.ssq, p.c1.cout_pad, V, nullptr, nullptr, a1);
@@ -686,9 +696,11 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
     const int nb_act = cdiv(P, 256 * ACT_U);
     const dim3 grid(nb_act + (sparse1 ? 0 : cdiv(N, 256)), Gact, f.B);
     if (h2)
-      LION_LAUNCH(f.c, k_act_grid<true>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N);
+      LION_LAUNCH(f.c, k_act_grid<true>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N, mask1,
+                  p.c1.bias);
     else
-      LION_LAUNCH(f.c, k_act_grid<false>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N);
+      LION_LAUNCH(f.c, k_act_grid<false>, grid, 256, 0, raw1, act1, a1, Gout, p.cout, rp, P, nb_act, vp->ppos, g_in, Gin, N, mask1,
+                  p.c1.bias);
   }
   stamp(f.c, f.c->stream, " act1");
   // conv2 -> (stats) -> AdaGN + SE folded into one affine
@@ -1323,6 +1335,11 @@ extern "C" int lion_ctx_set_conv_whole_slabs(LionCtx* h, int on) {
   h->c.conv_whole_slabs = on != 0;
   return 0;
 }
+extern "C" int lion_ctx_set_sparse_conv1_dense(LionCtx* h, int on) {
+  LION_REQUIRE(h, "lion_ctx_set_sparse_conv1_dense: null context");
+  h->c.sparse_conv1_dense = on != 0;
+  return 0;
+}
 extern "C" unsigned lion_ctx_generation(LionCtx* h) { return h ? h->c.generation : 0; }
 extern "C" int lion_ctx_timeline(LionCtx* h, unsigned long long* t_ns, char* names, int max_entries) {
   LION_REQUIRE(h && t_ns && names && max_entries >= 0, "lion_ctx_timeline: null argument");
@@ -1678,11 +1695,11 @@ extern "C" int lion_pvconv_conv1_probe(LionModel* h, const float* features, cons
     VoxPrep* vp;
     LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
     Conv1Out c1;
-    LION_TRY(pvconv_conv1(f, p, x, vp, path, c1, [] { return 0; }));
+    LION_TRY(pvconv_conv1(f, p, x, vp, path, true, c1, [] { return 0; }));
     // the dense path scattered into the context's zero grid: zero those voxels again (k_act_grid's extra blocks alone)
     if (!c1.sparse)
       LION_LAUNCH(f.c, k_act_grid<false>, dim3(cdiv(N, 256), Gout, B), 256, 0, c1.raw, nullptr, AffSrc{}, Gout, p.cout, rp, P, 0,
-                  vp->ppos, c1.g_in, p.cin / 4, N);
+                  vp->ppos, c1.g_in, p.cin / 4, N, nullptr, nullptr);
     LION_LAUNCH(f.c, k_vg_to_cm, dim3(cdiv(r * r * r, 256), Gout, B), 256, 0, c1.raw, out, p.cout, Gout, r);
     if (!f.c->dry) {
       LION_CHECK_CUDA(cudaMemcpy2DAsync(gn_sum, sizeof(double) * p.cout, c1.ssum, sizeof(double) * p.c1.cout_pad,
@@ -1692,6 +1709,27 @@ extern "C" int lion_pvconv_conv1_probe(LionModel* h, const float* features, cons
       if (path_taken) *path_taken = c1.sparse ? 2 : 1;
     }
     return check_launch(f.c, "lion_pvconv_conv1_probe");
+  });
+}
+
+// The sparse first convolution's vgrid and activity mask (include/lion_b200.h)
+extern "C" int lion_pvconv_conv1_mask_probe(LionModel* h, const float* features, const float* coords, int* vgrid, unsigned* mask,
+                                            int B, int N, void* stream) {
+  LION_REQUIRE(h && h->m.kind == LION_KIND_PVCONV, "lion_pvconv_conv1_mask_probe: not a pvconv model");
+  LION_REQUIRE(features && coords && vgrid && mask && B > 0 && N > 0, "lion_pvconv_conv1_mask_probe: bad arguments");
+  Model* m = &h->m;
+  return two_pass(m, stream, B, [&](Fwd& f) -> int {
+    const PVConvBlk& p = m->block->pv;
+    const int r = p.r, rp = r + 2, P = rp * rp * rp;
+    PF x = to_pf(f, features, m->desc[0], N);
+    float4* c4 = to_c4(f, coords, N);
+    VoxPrep* vp;
+    LION_TRY(get_vox(f, f.c->stream, c4, N, r, &vp));
+    Conv1Out c1;
+    LION_TRY(pvconv_conv1(f, p, x, vp, 2, false, c1, [] { return 0; }));
+    LION_TRY(memcpy_d2d(f.c, vgrid, vp->vgrid, sizeof(int) * (size_t)B * P));
+    LION_TRY(memcpy_d2d(f.c, mask, c1.mask, sizeof(unsigned) * (size_t)B * cdiv(r * r * r, 32)));
+    return check_launch(f.c, "lion_pvconv_conv1_mask_probe");
   });
 }
 

@@ -164,6 +164,10 @@ __global__ void k_scatter_compact(const float4* __restrict__ feat, const int* __
 // (one dense GEMM over the compact list, k_ygemm in sparse_conv.cu); here every interior output voxel p sums,
 // in ascending tap order, the rows y[vgrid[p + off(t)]][t] of its occupied neighbours -- each y row is read exactly
 // once -- adds the bias, stores the raw convolution output and accumulates the GroupNorm statistics.  Deterministic.
+// A voxel none of whose 27 neighbours is occupied ("inactive": 67-84 % of the voxels of the prior's latent points at r = 32)
+// holds exactly the bias: bit j of mask[b][w] is set when voxel 32 w + j is active, and only active voxels are stored
+// unless store_all (k_act_grid substitutes the bias for the rest; probes read the whole grid).  The GroupNorm sums
+// still cover every voxel.
 //   one warp = 32 consecutive interior voxels; accumulators [32][C] in shared memory; C <= 64 (2 channels per lane)
 //   grid = (ceil(r^3 / (32 * warps)), B), block = 32 * warps, dynamic smem = warps * (32 * (C + 2) floats + SPG_LIST int2)
 constexpr int SPG_LIST = 256;      // contribution-list entries per warp (packed: v << 10 | tap << 5 | voxel-in-warp)
@@ -206,7 +210,7 @@ template <int C>
 __global__ void __launch_bounds__(128)
 k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict__ vgrid, const float* __restrict__ bias,
                      float4* __restrict__ out, double* __restrict__ ssum, double* __restrict__ ssq, int stat_stride,
-                     int r, int Nrows) {
+                     int r, int Nrows, unsigned* __restrict__ mask, bool store_all) {
   static_assert(C == 32 || C == 64, "two (or one) channels per lane");
   constexpr int CPL = C / 32;                     // channels per lane
   constexpr int PITCH = C + 2;
@@ -242,17 +246,22 @@ k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict
   // consumed in that order: the accumulation order per output voxel is ascending t whatever the batching
   unsigned* list = reinterpret_cast<unsigned*>(s_acc + (size_t)nw * 32 * PITCH) + wid * SPG_LIST;
   int n = 0;
+  bool any = false;                               // this lane's voxel has an occupied neighbour
 #pragma unroll
   for (int t = 0; t < 27; ++t) {
     const int v = nb[t];
     const unsigned m = __ballot_sync(0xffffffffu, v >= 0);
+    any |= v >= 0;
     if (n + 32 > SPG_LIST) { spg_flush<C>(acc, list, n, yb, ldy, lane); n = 0; }
     if (v >= 0) list[n + __popc(m & ((1u << lane) - 1u))] = ((unsigned)v << 10) | ((unsigned)t << 5) | (unsigned)lane;
     n += __popc(m);
   }
   spg_flush<C>(acc, list, n, yb, ldy, lane);
+  const int word = (int)blockIdx.x * nw + wid;
+  const unsigned active = __ballot_sync(0xffffffffu, any);
+  if (lane == 0 && word * 32 < V) mask[(size_t)b * ((V + 31) / 32) + word] = active;
   // store (PF/VG layout: consecutive lanes = consecutive z) and statistics
-  if (live) {
+  if (live && (store_all || any)) {
 #pragma unroll
     for (int g = 0; g < C / 4; ++g) {
       const float* a = acc + lane * PITCH + g * 4;
@@ -263,7 +272,7 @@ k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict
 #pragma unroll
   for (int k = 0; k < CPL; ++k) { cs[0][k] = cs[1][k] = 0.0f; cq[0][k] = cq[1][k] = 0.0f; }
   // (signed: with the unsigned blockIdx.x the difference wraps for the warps past V, and min() then counts 32 rows)
-  const int nlive = max(0, min(32, V - ((int)blockIdx.x * nw + wid) * 32));
+  const int nlive = max(0, min(32, V - word * 32));
   for (int j = 0; j < nlive; j += 2) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -609,9 +618,13 @@ __device__ __forceinline__ float4 h8_pack(float4 a, float4 b) {
 // Blocks with blockIdx.x >= nb_act do k_unscatter's job instead (us_ppos != null): they restore the all-zero
 // invariant of the persistent scatter grid that the first convolution has finished reading by now (one launch less
 // per PVConv on the critical path); block (x, y, z) zeroes its 256 points in groups y, y + gridDim.y, ... < us_G.
+// mask (the sparse first convolution's activity bits, k_sparse_conv_gather; null = read every interior position): an
+// interior position whose bit is clear is neither read nor recomputed -- its input is exactly bias (null = 0), and the
+// block computes that position's output once, with the same expression.
 template <bool F16>
 __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ out, AffSrc aff, int G, int C, int rp, int P,
-                           int nb_act, const int* __restrict__ us_ppos, float4* __restrict__ us_grid, int us_G, int us_N) {
+                           int nb_act, const int* __restrict__ us_ppos, float4* __restrict__ us_grid, int us_G, int us_N,
+                           const unsigned* __restrict__ mask, const float* __restrict__ bias) {
   constexpr int NG = F16 ? 2 : 1;                       // fp32 input groups per output row
   int b = blockIdx.z, g = blockIdx.y;
   if ((int)blockIdx.x >= nb_act) {
@@ -631,8 +644,21 @@ __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ o
   const float4* src = in + ((size_t)b * G + NG * g) * P;
   float4* dst = out + ((size_t)b * (G / NG) + g) * P;
   const int p0 = blockIdx.x * (blockDim.x * ACT_U) + threadIdx.x;
+  const int r = rp - 2;
+  const unsigned* mb = mask ? mask + (size_t)b * ((r * r * r + 31) / 32) : nullptr;
+  float4 cst = make_float4(0.f, 0.f, 0.f, 0.f);          // the output of an inactive position
+  if (mask) {
+    float4 bv[NG];
+#pragma unroll
+    for (int k = 0; k < NG; ++k) {
+      const int c0 = (NG * g + k) * 4;
+      bv[k] = bias ? make_float4(bias[c0], bias[c0 + 1], bias[c0 + 2], bias[c0 + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if constexpr (F16) cst = h8_pack(f4_swish(f4_affine(bv[0], s[0], t[0])), f4_swish(f4_affine(bv[1], s[1], t[1])));
+    else cst = f4_tf32(f4_swish(f4_affine(bv[0], s[0], t[0])));
+  }
   float4 v[ACT_U][NG];
-  bool interior[ACT_U];
+  bool interior[ACT_U], active[ACT_U];
   // p -> (x, y, z) by multiply-high with m = ceil(2^32 / rp) (exact while p * rp < 2^32): the four positions of a thread
   // cost one integer division instead of sixteen -- at 1 float4 per clock per SM this pass is instruction-bound, not
   // HBM-bound, once the index arithmetic and an IEEE division per Swish are in the loop
@@ -643,22 +669,29 @@ __global__ void k_act_grid(const float4* __restrict__ in, float4* __restrict__ o
     const int q = (int)__umulhi((unsigned)p, rp_m), x = (int)__umulhi((unsigned)q, rp_m);
     const int z = p - q * rp, y = q - x * rp;
     interior[u] = p < P && z >= 1 && z <= rp - 2 && y >= 1 && y <= rp - 2 && x >= 1 && x <= rp - 2;
+    active[u] = interior[u];
+    if (mb && interior[u]) {
+      const int qi = ((x - 1) * r + (y - 1)) * r + (z - 1);      // interior voxel index, as the gather numbers it
+      active[u] = (__ldg(mb + (qi >> 5)) >> (qi & 31)) & 1u;
+    }
 #pragma unroll
     for (int k = 0; k < NG; ++k) {
       v[u][k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (interior[u]) v[u][k] = __ldcs(src + (size_t)k * P + p);   // read once: streaming
+      if (active[u]) v[u][k] = __ldcs(src + (size_t)k * P + p);     // read once: streaming
     }
   }
 #pragma unroll
   for (int u = 0; u < ACT_U; ++u) {
     int p = p0 + u * blockDim.x;
     if (p < P) {
-      float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (interior[u]) {                                 // sole consumer: the second 3x3x3 convolution
-        if constexpr (F16) r = h8_pack(f4_swish(f4_affine(v[u][0], s[0], t[0])), f4_swish(f4_affine(v[u][1], s[1], t[1])));
-        else r = f4_tf32(f4_swish(f4_affine(v[u][0], s[0], t[0])));
+      float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (active[u]) {                                   // sole consumer: the second 3x3x3 convolution
+        if constexpr (F16) o = h8_pack(f4_swish(f4_affine(v[u][0], s[0], t[0])), f4_swish(f4_affine(v[u][1], s[1], t[1])));
+        else o = f4_tf32(f4_swish(f4_affine(v[u][0], s[0], t[0])));
+      } else if (interior[u]) {
+        o = cst;
       }
-      dst[p] = r;
+      dst[p] = o;
     }
   }
 }
