@@ -38,6 +38,15 @@ int lion_ctx_set_conv_whole_slabs(LionCtx* ctx, int on);
  * outputs are bitwise the same either way); 0 restores the default, which stores and reads only voxels with an occupied
  * neighbour.  Returns 0. */
 int lion_ctx_set_sparse_conv1_dense(LionCtx* ctx, int on);
+/* For tests: how the second convolution of every later PVConv whose first convolution ran sparse treats its 64-row
+ * blocks whose every input is the inactive-voxel value or a halo zero.  0 (default): their copies and MMAs are skipped
+ * and their outputs and GroupNorm sums come from the 27 border-class values; 1: every block is computed; 2: as 0, with
+ * the output grid filled with NaNs first (rows that are not stored then stay NaN).  The outputs are bitwise the same in
+ * all three.  Returns 0, or an error for another mode. */
+int lion_ctx_set_conv2_class_mode(LionCtx* ctx, int mode);
+/* The blocks that the last such convolution on this context found class-valued (*flagged) out of those it examined
+ * (*total: shapes x two per 128-row tile).  Synchronises the device.  Returns 0. */
+int lion_ctx_last_conv2_class_blocks(LionCtx* ctx, long long* flagged, long long* total);
 /* Scratch-arena generation: bumped whenever a call had to re-allocate the per-device arena or zero grid.  A CUDA graph
  * captured on this context has the arena addresses baked in; it must not be replayed once the generation changed
  * (lion_b200._lib.capture_graph checks this and raises). */

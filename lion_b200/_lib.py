@@ -35,6 +35,8 @@ def _proto(lib):
         "lion_ctx_last_conv_stage_taps": (P(vp), i),
         "lion_ctx_set_conv_whole_slabs": (P(vp, i), i),
         "lion_ctx_set_sparse_conv1_dense": (P(vp, i), i),
+        "lion_ctx_set_conv2_class_mode": (P(vp, i), i),
+        "lion_ctx_last_conv2_class_blocks": (P(vp, vp, vp), i),
         "lion_ctx_arena_bytes": (P(vp), sz),
         "lion_ctx_generation": (P(vp), C.c_uint),
         "lion_ctx_timeline": (P(vp, vp, vp, i), i),

@@ -78,6 +78,12 @@ struct Ctx {
   // set by tests only (lion_ctx_set_sparse_conv1_dense): the sparse first convolution stores every voxel of its output
   // and the activation pass reads every interior position (no activity mask)
   bool sparse_conv1_dense = false;
+  // set by tests only (lion_ctx_set_conv2_class_mode): 0 = the second convolution of a PVConv whose first one ran sparse
+  // skips its class-valued blocks, 1 = it computes every block, 2 = it skips them and its output grid is filled with NaNs
+  // first (no reader may touch an unstored row)
+  int conv2_class_mode = 0;
+  unsigned long long* d_cls_count = nullptr;   // class-valued blocks flagged by the last k_conv2_flags (device)
+  long long cls_blocks = 0;                    // the blocks it examined
   // LION_TIMELINE=1 (diagnostic, tools/timeline_step.py): %globaltimer stamps dropped into both streams at block
   // boundaries -- this image has no nsys, and a step's critical path across the two streams is not visible otherwise
   unsigned long long* d_stamps = nullptr;

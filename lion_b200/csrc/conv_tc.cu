@@ -100,6 +100,15 @@ struct Params {
   int tps;               // taps per weight stage: tpg (whole slabs), or 3 (3x3x3 slabs streamed in 3-tap parts)
   const unsigned char* occ;   // 64-row occupancy flags of the input (sparse first conv of a PVConv) or null
   int occ_stride;
+  // 3x3x3 row tiles: one byte per 64-row block of [p_begin, p_end) per shape ([B][cls_stride], block k = rows p_begin +
+  // 64 k ..), set where every operand of every interior row is a per-channel constant or a halo zero (k_conv2_flags), or
+  // null.  A flagged block's outputs are its rows' border-class values, cls [B][cout_pad / 4][5^3]: the same convolution
+  // of a 3x3x3 grid of those constants (row ((cx+1) * 5 + cy+1) * 5 + cz+1 for the low / interior / high class 0 / 1 / 2
+  // of x, y and z).  Its MMAs and copies are skipped; its rows are stored only when cls_store.
+  const unsigned char* cls_flag;
+  int cls_stride;
+  const float4* cls;
+  int cls_store;
   // pooled 1x1 (last layer of a set-abstraction MLP): instead of the [rows][C] result, write per 32 consecutive rows (the
   // neighbours of one centre) the per-channel minimum and maximum, pool_mm[b][C/4][rows/32][2][4].  AdaGN's affine is
   // monotonic and Swish is quasi-convex (one minimum), so max_i swish(s*x_i + t) = max(swish(s*min + t), swish(s*max + t)):
@@ -189,6 +198,9 @@ __device__ __forceinline__ Items make_items(long long U, int ntile_total, int B,
   }
   return it;
 }
+
+// border class of coordinate v (1 .. r) of a 3x3x3 row tile: 0 low, 1 interior, 2 high (Params::cls)
+__device__ __forceinline__ int cls_of(int v, int r) { return v <= 1 ? 0 : (v >= r ? 2 : 1); }
 
 // GroupNorm statistics in the row tiles' grouping, shared by k_conv_tc's epilogue and k_conv_stats so that both sum
 // alike: per fragment a shuffle tree over the warp's 8 row pairs, per-warp fp32 partials in s_stat [8 consumer warps]
@@ -316,6 +328,14 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
       // lane l keeps (shape, row tile) of the item's tile l: one division per item, a shuffle per stage
       int my_b = 0, my_t = 0;
       if (lane < ntile) { const int vl = (int)v0 + lane; my_b = vl / ntile_total; my_t = vl - my_b * ntile_total; }
+      // tiles with an operand to copy: all but those whose two 64-row blocks are both class-valued (the consumers
+      // compute the same set and skip the same ring slots)
+      unsigned live = (1u << ntile) - 1u;
+      if (!BLK && P.cls_flag) {
+        const unsigned char* fl = P.cls_flag + (size_t)my_b * P.cls_stride + 2 * my_t;
+        live = __ballot_sync(0xffffffffu, lane < ntile && !(__ldg(fl) && __ldg(fl + 1)));
+      }
+      if (!live) continue;                             // every output of the item is a class value: no weights either
       for (int cc = 0; cc < P.nchunk; ++cc) {
         const int kg_real = min(KG, P.Gin - cc * KG);
         const size_t grp_lane = (size_t)(cc * KG + (lane < kg_real ? lane : 0));
@@ -328,6 +348,7 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
           const float* slab = wsrc + (size_t)(cc * P.ntg + tg) * slab_floats;
           copy_weights(slab);
           for (int j = 0; j < ntile; ++j) {
+            if (!((live >> j) & 1u)) continue;
             const int bj = __shfl_sync(0xffffffffu, my_b, j), tj = __shfl_sync(0xffffffffu, my_t, j);
             // row tiles: the tile's 128 rows (3x3x3: plus rp+1 halo rows on each side, shifted to x-plane tg).  Interior
             // blocks: the window of block group tj under tap group tg, from one row before
@@ -426,7 +447,24 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
       // until the group of its last part has completed.
       int pend_a = -1, pend_b = -1;
       bool skip[BLK ? 1 : GT];
-      for (int cc = 0; cc < P.nchunk; ++cc) {
+      // row tiles with class-valued blocks (Params::cls_flag): `live` tiles have an A stage (the producer's set), `mine`
+      // those whose block of this warpgroup is computed
+      unsigned live = (1u << ntile) - 1u, mine = ~0u;
+      if (!BLK && P.cls_flag) {
+        live = 0u; mine = 0u;
+#pragma unroll
+        for (int j = 0; j < GT; ++j) {
+          if (j < ntile) {
+            const long long vj = v0 + j;
+            const int bj = (int)(vj / ntile_total), tj = (int)(vj - (long long)bj * ntile_total);
+            const unsigned char* fl = P.cls_flag + (size_t)bj * P.cls_stride + 2 * tj;
+            const bool f0 = __ldg(fl) != 0, f1 = __ldg(fl + 1) != 0;
+            if (!(f0 && f1)) live |= 1u << j;
+            if (!(wg ? f1 : f0)) mine |= 1u << j;
+          }
+        }
+      }
+      for (int cc = 0; cc < (live ? P.nchunk : 0); ++cc) {
         for (int tg = 0; tg < P.ntg; ++tg) {
           const uint32_t sa0 = sa, pa0 = pa;             // A stage of the slab's first tile
 #pragma unroll
@@ -438,11 +476,12 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
             sa = sa0; pa = pa0;
 #pragma unroll
             for (int j = 0; j < (BLK ? 1 : GT); ++j) {
-              if (j < ntile) {
+              if ((live >> j) & 1u) {
                 if (s == 0) {
                   mbar_wait<SETREG>(bar_full_a + 8 * sa, pa);
-                  skip[j] = s_skip[sa] != 0;
-                  if (skip[j]) { int st = (int)sa; release(st, bar_empty_a); }   // all-zero input slab: nothing to accumulate
+                  // all-zero input slab (nothing to accumulate), or this warpgroup's block is class-valued
+                  skip[j] = s_skip[sa] != 0 || !((mine >> j) & 1u);
+                  if (skip[j]) { int st = (int)sa; release(st, bar_empty_a); }
                 }
                 if (!skip[j]) {
                   const uint32_t a_addr = a_ring + sa * (uint32_t)P.a_stage_bytes;
@@ -472,6 +511,11 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
             }
             if (issued) pend_b = (int)sb;                // the group in flight still reads this weight stage
             else { int st = (int)sb; release(st, bar_empty_b); }
+            if ((live & ~mine) && pend_b >= 0) {          // see conv_tc_run: class-valued blocks and the A ring
+              wg_wait<0>();
+              release(pend_a, bar_empty_a);
+              release(pend_b, bar_empty_b);
+            }
             if (++sb == B_STAGES) { sb = 0; pb ^= 1; }
           }
         }
@@ -504,6 +548,23 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
             in_lo = p_lo < P.p_end; in_hi = p_hi < P.p_end;
             ok_lo = in_lo; ok_hi = in_hi;
             if (TPG != 1) halo_mask(p_lo, P.rp, ok_lo, ok_hi);   // halo rows are stored as zeros
+            if (!((mine >> j) & 1u)) {
+              // class-valued block: the accumulators take the border-class values of their rows (the bias included)
+              // and the statistics below sum them as they would the computed ones
+              const float4* cb = P.cls + (size_t)b * (P.cout_pad / 4) * 125 + n0 / 4;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int p = h ? p_hi : p_lo, x = p / (P.rp * P.rp), y = (p / P.rp) % P.rp, z = p % P.rp;
+                const int row = ((cls_of(x, P.r) + 1) * 5 + cls_of(y, P.r) + 1) * 5 + cls_of(z, P.r) + 1;
+                // channels n0 + 8 i + c_lo, + 1: group n0 / 4 + 2 i + (lane & 3) / 2, floats 2 (lane & 1), + 1
+                const float* src = reinterpret_cast<const float*>(cb + ((lane & 3) >> 1) * 125 + row) + 2 * (lane & 1);
+#pragma unroll
+                for (int i = 0; i < NT / 8; ++i) {
+                  const float2 v = __ldg(reinterpret_cast<const float2*>(src + (size_t)2 * 125 * 4 * i));
+                  acc[j][4 * i + 2 * h] = v.x; acc[j][4 * i + 2 * h + 1] = v.y;
+                }
+              }
+            }
           } else {
             // fragment row i of block k is voxel (y0 + i / 8, z0 + i % 8): this thread's rows are y-lines y0 + 2 wq
             // and y0 + 2 wq + 1 at z0 + lane / 4.  Rows past r (a last block of an r that is not a multiple of 8) are
@@ -514,11 +575,13 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
             ok_lo = y <= P.r && z <= P.r; ok_hi = y + 1 <= P.r && z <= P.r;
             in_lo = ok_lo; in_hi = ok_hi;
           }
+          const bool cmp = (mine >> j) & 1u, st = cmp || P.cls_store;   // computed block / rows stored
 #pragma unroll
           for (int i = 0; i < NT / 8; ++i) {
             const int col = 8 * i + c_lo;
-            const float x0 = ok_lo ? acc[j][4 * i + 0] + s_bias[col] : 0.0f, x1 = ok_lo ? acc[j][4 * i + 1] + s_bias[col + 1] : 0.0f;
-            const float x2 = ok_hi ? acc[j][4 * i + 2] + s_bias[col] : 0.0f, x3 = ok_hi ? acc[j][4 * i + 3] + s_bias[col + 1] : 0.0f;
+            float x0 = acc[j][4 * i + 0], x1 = acc[j][4 * i + 1], x2 = acc[j][4 * i + 2], x3 = acc[j][4 * i + 3];
+            if (cmp) { x0 += s_bias[col]; x1 += s_bias[col + 1]; x2 += s_bias[col]; x3 += s_bias[col + 1]; }
+            x0 = ok_lo ? x0 : 0.0f; x1 = ok_lo ? x1 : 0.0f; x2 = ok_hi ? x2 : 0.0f; x3 = ok_hi ? x3 : 0.0f;
             if (P.ssum) stat_add<NT>(s_stat, cw, lane, col, x0, x1, x2, x3);
             if (TPG == 1 && P.pool_mm) {                 // all rows valid (rows % 128 == 0)
               const float mn0 = red8<1>(fminf(x0, x2)), mn1 = red8<1>(fminf(x1, x3));
@@ -534,8 +597,8 @@ __global__ void __launch_bounds__(conv_threads(BPW), 1) k_conv_tc(Params P) {
               const int g = (n0 + 8 * i + (lane & 2) * 2) >> 2;
               if (g < P.Gout_store) {
                 float4* o = P.out + ((size_t)b * P.Gout_store + g) * P.rows;
-                if (!odd && in_lo) o[p_lo] = make_float4(x0, x1, y0, y1);
-                if (odd && in_hi) o[p_hi] = make_float4(y0, y1, x2, x3);
+                if (!odd && in_lo && st) o[p_lo] = make_float4(x0, x1, y0, y1);
+                if (odd && in_hi && st) o[p_hi] = make_float4(y0, y1, x2, x3);
               }
             }
           }
@@ -718,6 +781,9 @@ int conv_tc_prepare_f16(Model* m, ConvW& w) {
   return 0;
 }
 
+// whether conv_tc_run computes this 3x3x3 convolution on row tiles, the only tiling that takes class-valued blocks
+bool conv_tc_row_tiles_3x3(const ConvW& w) { return w.tc.w && w.ntaps == 27 && w.tc.NT <= 64; }
+
 bool conv_tc_usable(const ConvW& w, const ConvGeom& geo) {
   if (!w.tc.w) return false;
   if (geo.ntaps != w.ntaps) return false;
@@ -741,6 +807,7 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   const int slab_bytes = tpg * KG * NT * 16;     // the weights of one (channel chunk, x-plane)
   P.B = B;
   P.occ = geo.occ; P.occ_stride = geo.occ_stride;
+  P.cls_flag = geo.cls_flag; P.cls_stride = geo.cls_stride; P.cls = geo.cls; P.cls_store = geo.cls_store ? 1 : 0;
   const size_t fixed = tc::smem_fixed(NT, tpg);
   // 3x3x3 with N = 128 runs on interior blocks (BLK); its chunking (16 channels) and so every output's accumulation
   // order are those of the row tiles.  N <= 64 keeps the 128-row tiles: its 32-channel chunks leave no room for a
@@ -861,6 +928,15 @@ int conv_tc_run(Ctx* c, const ConvW& w, const float4* in, int Gin, float4* out, 
   // consumers wait for each other (4-tile items on the 6-stage ring of N = 32 with 32-channel chunks).  Without the flags
   // the all-zero slabs are multiplied instead, which adds exact zeros.  (Block groups retire every slab.)
   if (!blk && P.occ && a_stages < 2 * P.G) P.occ = nullptr;
+  // Class-valued blocks (Params::cls_flag): the producer copies, and the consumers wait for, the A stages of the tiles
+  // with a computed block only.  A warpgroup with a class-valued block in an item retires its MMAs at the end of every
+  // slab, so it holds an A stage only while it waits for the stages of the same slab's later tiles, fewer than G: an A
+  // ring of G stages cannot deadlock (test_conv2_const_skip_cpu.py simulates the protocol).  On a shallower ring every
+  // block is computed, which gives the same bits.
+  if (P.cls_flag && (blk || w.ntaps != 27 || P.occ || 2 * ntile > P.cls_stride)) {
+    set_error("conv_tc: class-valued blocks are for 3x3x3 row tiles of a dense input"); return LION_ERR_ARG;
+  }
+  if (a_stages < P.G) P.cls_flag = nullptr;
   size_t smem = (size_t)a_stages * P.a_stage_bytes + (size_t)b_stages * P.b_stage_bytes + fixed;
   if (smem > 227 * 1024) { set_error("conv_tc: %zu bytes of shared memory needed", smem); return LION_ERR_ARG; }
   // persistent, at most one CTA per SM: the fewest CTAs that still reach the minimal maximum of tiles per CTA

@@ -195,12 +195,19 @@ struct ConvGeom {
   int p_begin, p_end;
   const unsigned char* occ;   // optional 64-row occupancy flags of the INPUT ([B][occ_stride]); null = dense
   int occ_stride;
+  // optional class-valued 64-row blocks of a 3x3x3 row-tile convolution's output and their values (conv_tc.cu:
+  // Params::cls_flag); cls_store: store those rows too
+  const unsigned char* cls_flag;
+  int cls_stride;
+  const float4* cls;
+  bool cls_store;
 };
 
 // conv_tc.cu
 int conv_tc_prepare(Model* m, ConvW& w);
 int conv_tc_prepare_f16(Model* m, ConvW& w);
 bool conv_tc_usable(const ConvW& w, const ConvGeom& geo);
+bool conv_tc_row_tiles_3x3(const ConvW& w);
 // sparse first convolution, GEMM half (sparse_conv.cu)
 bool ygemm_usable(const ConvW& y);
 int ygemm_run(Ctx* c, const ConvW& y, const float4* xc, float* out, int ld, const int* nocc, int B, int N);

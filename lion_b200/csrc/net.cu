@@ -657,6 +657,42 @@ static int pvconv_conv1(Fwd& f, const PVConvBlk& p, PF feat, const VoxPrep* vp, 
   return 0;
 }
 
+// The second convolution of a PVConv whose first one ran sparse reads, at every interior voxel without an occupied
+// neighbour (mask1 clear), the one value per (shape, channel) that k_act_grid writes there.  An output voxel none of
+// whose 27 neighbours is active is then a function of its border class alone (low, interior or high in each of x, y and
+// z): k_conv2_flags marks the row tiles' 64-row blocks made only of such voxels, and the same kernel instantiation
+// convolves a 3x3x3 grid of that value (k_act_grid with an all-clear mask, so the very same bits) into the 27 class
+// values per channel.  The tensor cores give an output element the same bits whatever its row, so the convolution
+// can skip those blocks' copies and MMAs and take their outputs and GroupNorm sums from the class values
+// (conv_tc.cu: Params::cls_flag) without changing a bit.  Flagged rows are stored in probe mode only: the
+// devoxelisation reads trilinear corners within one voxel of a point, which are active.
+static int conv2_classes(Fwd& f, const PVConvBlk& p, const VoxPrep* vp, const unsigned* mask1, const float4* raw1,
+                         const AffSrc& a1, bool h2, ConvGeom& geo) {
+  const int r = p.r, rp = r + 2, Gout = p.cout / 4, Gc = p.c2.cout_pad / 4, Gact = h2 ? Gout / 2 : Gout;
+  const int nblk = 2 * cdiv(r * rp * rp, 128);        // two per row tile
+  if (nblk > vp->occ_stride) { set_error("conv2 classes: %d blocks exceed the flag stride %d", nblk, vp->occ_stride); return LION_ERR_STATE; }
+  unsigned char* flags = f.c->alloc_n<unsigned char>((size_t)f.B * vp->occ_stride);
+  unsigned* zmask = f.c->alloc_n<unsigned>((size_t)f.B);
+  LION_TRY(memset_async(f.c, f.c->d_cls_count, 0, sizeof(unsigned long long)));
+  LION_LAUNCH(f.c, k_conv2_flags, dim3(cdiv(nblk, 8), f.B), 256, 0, mask1, r, nblk, flags, vp->occ_stride, zmask, f.c->d_cls_count);
+  f.c->cls_blocks = (long long)f.B * nblk;
+  // the class grid (r = 3, 125 rows per channel group); its row tile reads from 31 rows before to 59 past them, whose
+  // outputs are not kept
+  const int CP = 125, guard = 64;
+  float4* cg = f.c->alloc_n<float4>((size_t)f.B * Gact * CP + 2 * guard) + guard;
+  if (h2)
+    LION_LAUNCH(f.c, k_act_grid<true>, dim3(1, Gact, f.B), 256, 0, raw1, cg, a1, Gout, p.cout, 5, CP, 1, nullptr, nullptr, 0, 0,
+                zmask, p.c1.bias);
+  else
+    LION_LAUNCH(f.c, k_act_grid<false>, dim3(1, Gact, f.B), 256, 0, raw1, cg, a1, Gout, p.cout, 5, CP, 1, nullptr, nullptr, 0, 0,
+                zmask, p.c1.bias);
+  LION_TRY(check_launch(f.c, "conv2 classes"));
+  float4* cls = f.c->alloc_n<float4>((size_t)f.B * Gc * CP);
+  LION_TRY(run_conv(f, p.c2, cg, Gact, cls, Gc, nullptr, nullptr, geom_grid(3), nullptr, h2));
+  geo.cls_flag = flags; geo.cls_stride = vp->occ_stride; geo.cls = cls; geo.cls_store = f.pv != nullptr;
+  return 0;
+}
+
 // PVConv: features PF [cin] + coords -> dst PF (cout) at (Gd, g_off)
 static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, float4* dst, int Gd, int g_off) {
   int N = feat.R, r = p.r, rp = r + 2, P = rp * rp * rp, Gin = p.cin / 4, Gout = p.cout / 4;
@@ -706,8 +742,15 @@ static int pvconv_fwd(Fwd& f, const PVConvBlk& p, PF feat, const float4* c4, flo
   // conv2 -> (stats) -> AdaGN + SE folded into one affine
   float4* raw2 = alloc_vg(f, Gout, r);
   LION_TRY(poison_vg(f, raw2, Gout, r));
+  ConvGeom geo2 = geo;
+  // (r >= 3: at r <= 2 a voxel lies on both the low and the high border and has no single class)
+  if (mask1 && r >= 3 && f.c->conv2_class_mode != 1 && conv_tc_row_tiles_3x3(p.c2)) {
+    if (f.c->conv2_class_mode == 2 && !f.pv)
+      LION_TRY(memset_async(f.c, raw2, 0xff, sizeof(float4) * f.B * Gout * (size_t)P));
+    LION_TRY(conv2_classes(f, p, vp, mask1, raw1, a1, h2, geo2));
+  }
   AffSrc a2;
-  LION_TRY(conv_gn(f, p.c2, act1, Gact, raw2, Gout, geo, p.g2, V, p.se1, p.se2, a2, h2));
+  LION_TRY(conv_gn(f, p.c2, act1, Gact, raw2, Gout, geo2, p.g2, V, p.se1, p.se2, a2, h2));
   stamp(f.c, f.c->stream, " conv2");
   if (f.pv) {
     PvRecord& R = *f.pv;
@@ -1308,6 +1351,8 @@ extern "C" int lion_ctx_create(int device, LionCtx** out) {
   h->c.num_sms = prop.multiProcessorCount;
   h->c.l2_bytes = prop.l2CacheSize;
   LION_CHECK_CUDA(cudaStreamCreateWithFlags(&h->c.aux, cudaStreamNonBlocking));
+  LION_CHECK_CUDA(cudaMalloc(&h->c.d_cls_count, sizeof(unsigned long long)));
+  LION_CHECK_CUDA(cudaMemset(h->c.d_cls_count, 0, sizeof(unsigned long long)));
   { const char* e = getenv("LION_TIMELINE");
     if (e && atoi(e) != 0) LION_CHECK_CUDA(cudaMalloc(&h->c.d_stamps, LION_MAX_STAMPS * sizeof(unsigned long long))); }
   if (prop.major != 9 || prop.minor != 0) {
@@ -1324,6 +1369,7 @@ extern "C" int lion_ctx_destroy(LionCtx* h) {
   if (h->c.zgrid) cudaFree(h->c.zgrid);
   if (h->c.aux) cudaStreamDestroy(h->c.aux);
   if (h->c.d_stamps) cudaFree(h->c.d_stamps);
+  if (h->c.d_cls_count) cudaFree(h->c.d_cls_count);
   delete h;
   return 0;
 }
@@ -1338,6 +1384,20 @@ extern "C" int lion_ctx_set_conv_whole_slabs(LionCtx* h, int on) {
 extern "C" int lion_ctx_set_sparse_conv1_dense(LionCtx* h, int on) {
   LION_REQUIRE(h, "lion_ctx_set_sparse_conv1_dense: null context");
   h->c.sparse_conv1_dense = on != 0;
+  return 0;
+}
+extern "C" int lion_ctx_set_conv2_class_mode(LionCtx* h, int mode) {
+  LION_REQUIRE(h && mode >= 0 && mode <= 2, "lion_ctx_set_conv2_class_mode: null context or mode not 0-2");
+  h->c.conv2_class_mode = mode;
+  return 0;
+}
+extern "C" int lion_ctx_last_conv2_class_blocks(LionCtx* h, long long* flagged, long long* total) {
+  LION_REQUIRE(h && flagged && total, "lion_ctx_last_conv2_class_blocks: null argument");
+  unsigned long long n = 0;
+  LION_CHECK_CUDA(cudaSetDevice(h->c.device));
+  LION_CHECK_CUDA(cudaDeviceSynchronize());
+  LION_CHECK_CUDA(cudaMemcpy(&n, h->c.d_cls_count, sizeof(n), cudaMemcpyDeviceToHost));
+  *flagged = (long long)n; *total = h->c.cls_blocks;
   return 0;
 }
 extern "C" unsigned lion_ctx_generation(LionCtx* h) { return h ? h->c.generation : 0; }

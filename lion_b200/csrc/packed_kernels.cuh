@@ -293,6 +293,49 @@ k_sparse_conv_gather(const float* __restrict__ y, int ldy, const int* __restrict
   }
 }
 
+// Class-valued 64-row blocks of the second 3x3x3 convolution of a PVConv whose first one ran sparse.  Its input (k_act_grid
+// with the gather's activity mask) holds one value per (shape, channel) at every inactive interior voxel, so an output
+// voxel none of whose 27 neighbours is active depends on its border class only (conv_tc.cu: Params::cls_flag).  Block
+// k of shape b -- rows p_begin + 64 k .. + 63 of the row tiles' span [p_begin, p_end) = [rp^2, (rp-1) rp^2) -- is
+// flagged (flags[b][k] = 1) when no interior row of it lies within one voxel of an active one; the nblk blocks cover the
+// row tiles, those past p_end hold no interior row and are flagged.  One warp per block, two rows per lane.  Also
+// writes the all-clear activity mask of the 3x3x3 grid that computes the class values (zmask[b], one word) and adds
+// the flagged blocks to *count.
+__global__ void __launch_bounds__(256) k_conv2_flags(const unsigned* __restrict__ mask, int r, int nblk,
+                                                     unsigned char* __restrict__ flags, int stride,
+                                                     unsigned* __restrict__ zmask, unsigned long long* __restrict__ count) {
+  __shared__ int s_n;
+  const int b = blockIdx.y, lane = threadIdx.x & 31, k = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int rp = r + 2, p_end = (rp - 1) * rp * rp;
+  const unsigned* mb = mask + (size_t)b * ((r * r * r + 31) / 32);
+  if (threadIdx.x == 0) s_n = 0;
+  if (blockIdx.x == 0 && threadIdx.x == 0) zmask[b] = 0u;
+  __syncthreads();
+  bool hit = false;
+  if (k < nblk) {
+    for (int h = 0; h < 2; ++h) {
+      const int p = rp * rp + 64 * k + 32 * h + lane;
+      const int x = p / (rp * rp), y = (p / rp) % rp, z = p % rp;
+      if (p >= p_end || y < 1 || y > r || z < 1 || z > r) continue;
+      for (int dx = -1; dx <= 1; ++dx)
+        for (int dy = -1; dy <= 1; ++dy)
+          for (int dz = -1; dz <= 1; ++dz) {
+            const int xx = x + dx, yy = y + dy, zz = z + dz;
+            if (xx < 1 || xx > r || yy < 1 || yy > r || zz < 1 || zz > r) continue;
+            const int q = ((xx - 1) * r + (yy - 1)) * r + (zz - 1);
+            hit |= ((__ldg(mb + (q >> 5)) >> (q & 31)) & 1u) != 0;
+          }
+    }
+  }
+  const bool flag = !__any_sync(0xffffffffu, hit);
+  if (k < nblk && lane == 0) {
+    flags[(size_t)b * stride + k] = flag ? 1 : 0;
+    if (flag) atomicAdd(&s_n, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_n) atomicAdd(count, (unsigned long long)s_n);
+}
+
 // scatter-mean of PF rows into a (pre-zeroed) VG: one thread per (occupied voxel, channel group)
 // sums its points in ascending point order, each term scaled by 1/count first as the
 // reference does (vox.cu:65-68), and stores once.
